@@ -14,7 +14,9 @@
  *   6. the output is staged in a per-warp shared-memory ring and leaves the SM as coalesced
  *      16-byte stores (512 B per warp instruction); match sources come from the ring when they
  *      are recent and from global memory (L2) once flushed.
- * The block format and the presence of a dictionary are template parameters (decode_lz_block<UNITS, GHI, HAS_DICT>).
+ * The block format and the presence of a dictionary are template parameters (decode_lz_block<UNITS, GHI, HAS_DICT, LEAN>).
+ * The LEAN kernel instance decodes only RAW blocks and GLO blocks with raw or RLE literals and raw tokens, and defers
+ * every other block to the general instance (decode_job).
  * zxc_decode_stage.cuh holds the opt-in TMA flavour (sections staged by cp.async.bulk, ring flushed by bulk stores).
  * Overlapping matches (off < ml) use the period-`off` index instead of the reference's shuffle
  * tables (:197-413).  Output is written exactly (no wild-copy overshoot): none of the
@@ -75,7 +77,7 @@ typedef int32_t i32;
 #define FLAG_VERIFY 1u
 #define FLAG_UNITS_ON 4u
 #define FLAG_UNITS_OFF 8u
-#define FLAG_DEFERRED 2u /* only jobs whose status says D2_DEFER (left over by zxc_decode2_kernel) */
+#define FLAG_DEFERRED 2u /* only jobs whose status says D2_DEFER (left over by the lean instance or zxc_decode2_kernel) */
 #define D2_DEFER_STATUS ((i32)0x80000000)
 
 struct DecodeParams {
@@ -92,8 +94,8 @@ struct DecodeParams {
     u32 scratch_stride;
     u32 flags;
     u32 block_cap; /* largest decoded block size of this launch: sizes the per-warp scratch regions */
-    const u32* defer_list; /* FLAG_DEFERRED: job indices left over by zxc_decode2_kernel ... */
-    const u32* defer_count; /* ... how many; more than defer_cap means "scan the status array instead" */
+    u32* defer_list;  /* job indices the lean instance or zxc_decode2_kernel left to a FLAG_DEFERRED launch ... */
+    u32* defer_count; /* ... how many; more than defer_cap means "scan the status array instead" */
     u32 defer_cap;
 };
 
@@ -308,6 +310,8 @@ struct Sections {
     u32 enc_off;
 };
 
+/* LEAN: the caller has deferred every block with Huffman literals or tokens, so the PivCo decoder is not compiled in */
+template <bool LEAN>
 __device__ int parse_sections(const u8* pay, u32 comp, bool ghi, u32 cap, const u8* dict_huf, u8* scratch,
                               u32 block_cap, u32 lane, Sections& S) {
     /* scratch points at this warp's literal buffer; token buffer, Huffman work area follow */
@@ -335,7 +339,7 @@ __device__ int parse_sections(const u8* pay, u32 comp, bool ghi, u32 cap, const 
         if (enc_off > 1) return ZXC_ERROR_CORRUPT_DATA;
         const u8* p_data = pay + 12 + desc;
         const u32 avail = comp - 12 - desc;
-        if (enc_lit == 2 || enc_lit == 3) {
+        if (!LEAN && (enc_lit == 2 || enc_lit == 3)) {
             if (lit_comp > avail) return ZXC_ERROR_CORRUPT_DATA;
             if (n_lit != 0) {
                 if (n_lit > cap) return ZXC_ERROR_DST_TOO_SMALL;
@@ -383,7 +387,7 @@ __device__ int parse_sections(const u8* pay, u32 comp, bool ghi, u32 cap, const 
         if (enc_tok != 0 && enc_tok != 2) return ZXC_ERROR_CORRUPT_DATA;
         S.tok = p_data + lit_comp;
         S.offs = S.tok + tok_comp;
-        if (enc_tok == 2) { /* level 7: Huffman-coded tokens (:1019-1022) */
+        if (!LEAN && enc_tok == 2) { /* level 7: Huffman-coded tokens (:1019-1022) */
             if (n_seq + 32u > scr_tok_cap(block_cap) || tok_comp < 128) return ZXC_ERROR_CORRUPT_DATA;
             if (n_seq) {
                 const int rc = pivco_decode(S.tok, S.tok + 128, tok_comp - 128, tok_buf, n_seq, hw, cum, cum_words, lane);
@@ -686,8 +690,8 @@ __device__ __forceinline__ void balanced_copy_words(u32 ring_s, u32 m_items, u32
 /* ------------------------------------------------------------------------- */
 /* GHI and HAS_DICT are compile-time: the loop below sits at the kernel's register limit, and every branch and live
  * value it does not carry (the other block format's unpack, the dictionary pointer and its source classification)
- * is code the instruction cache does not hold and a register that is not spilled. */
-template <bool UNITS, bool GHI, bool HAS_DICT>
+ * is code the instruction cache does not hold and a register that is not spilled.  LEAN: see decode_job. */
+template <bool UNITS, bool GHI, bool HAS_DICT, bool LEAN>
 __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const u8* dict_in,
                                u32 dict_size_in, const u8* dict_huf, u8* scratch, u32 scratch_cap, u8* ring,
                                u32 lane, u32 P_flags) {
@@ -695,7 +699,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
     const u8* dict = HAS_DICT ? dict_in : (const u8*)0;
     const u32 dict_size = HAS_DICT ? dict_size_in : 0u;
     Sections S;
-    const int prc = parse_sections(pay, comp, ghi, cap, dict_huf, scratch, scratch_cap, lane, S);
+    const int prc = parse_sections<LEAN>(pay, comp, ghi, cap, dict_huf, scratch, scratch_cap, lane, S);
     if (prc != ZXC_OK) return prc;
     const u8* lit = S.lit;
     const u8* tok = S.tok;
@@ -1081,27 +1085,39 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
     return (int)(O + rem);
 }
 
-/* zxc_decompress_chunk_wrapper_body (zxc_decompress.c:1646-1695) for one job */
-template <bool UNITS, bool HAS_DICT>
+/* zxc_decompress_chunk_wrapper_body (zxc_decompress.c:1646-1695) for one job.
+ * LEAN: decode only what the bench-shaped frames are made of -- RAW blocks and GLO blocks with raw tokens and raw or
+ * RLE literals, in a launch without checksum verification -- and return D2_DEFER_STATUS for every other job, before
+ * anything is written to its output; the general instance decodes those.  The lean instance carries neither the PivCo
+ * Huffman decoder, the checksum nor the GHI body: a third of the code and a sixth of the spill traffic of the general
+ * one (DESIGN.md section 3d). */
+template <bool UNITS, bool HAS_DICT, bool LEAN = false>
 __device__ int decode_job(const DecodeParams& P, const zxc_b200_job_t& job, u8* scratch, u8* ring, u32 lane) {
     const u8* blk = P.src + job.src_off;
     u8* out = P.dst + job.dst_off;
-    if (job.src_len < 8) return ZXC_ERROR_SRC_TOO_SMALL;
+    if (job.src_len < 8) return LEAN ? D2_DEFER_STATUS : ZXC_ERROR_SRC_TOO_SMALL;
     const u32 type = blk[0];
     const u32 comp = ld32(blk + 3);
     const bool verify = (P.flags & FLAG_VERIFY) != 0;
+    if (LEAN) {
+        /* the 8-byte block header and, for GLO, bytes 8 (enc_lit) and 9 (enc_tok) of the 12-byte section header */
+        const bool whole = !verify && (u64)job.src_len >= 8ull + comp;
+        const bool take = whole && (type == BT_RAW || (type == BT_GLO && comp >= 12u && blk[8 + 9] == 0 && blk[8 + 8] <= 1));
+        if (!take) return D2_DEFER_STATUS;
+    }
     if ((u64)job.src_len < 8ull + comp + (verify ? 4u : 0u)) return ZXC_ERROR_SRC_TOO_SMALL;
     const u8* data = blk + 8;
-    if (verify) {
-        if (ld32(data + comp) != warp_checksum(data, comp, lane)) return ZXC_ERROR_BAD_CHECKSUM;
+    if constexpr (!LEAN) {
+        if (verify && ld32(data + comp) != warp_checksum(data, comp, lane)) return ZXC_ERROR_BAD_CHECKSUM;
     }
     switch (type) {
         case BT_GLO:
-            return decode_lz_block<UNITS, false, HAS_DICT>(data, comp, out, job.dst_cap, P.dict, P.dict_size, P.dict_huf,
-                                                           scratch, P.block_cap, ring, lane, P.flags);
+            return decode_lz_block<UNITS, false, HAS_DICT, LEAN>(data, comp, out, job.dst_cap, P.dict, P.dict_size,
+                                                                 P.dict_huf, scratch, P.block_cap, ring, lane, P.flags);
         case BT_GHI:
-            return decode_lz_block<UNITS, true, HAS_DICT>(data, comp, out, job.dst_cap, P.dict, P.dict_size, P.dict_huf,
-                                                          scratch, P.block_cap, ring, lane, P.flags);
+            if constexpr (LEAN) return D2_DEFER_STATUS; /* not reached: deferred above */
+            else return decode_lz_block<UNITS, true, HAS_DICT, false>(data, comp, out, job.dst_cap, P.dict, P.dict_size,
+                                                                      P.dict_huf, scratch, P.block_cap, ring, lane, P.flags);
         case BT_RAW:
             if (comp > job.dst_cap) return ZXC_ERROR_DST_TOO_SMALL;
             warp_copy(out, data, comp, lane);
@@ -1113,7 +1129,10 @@ __device__ int decode_job(const DecodeParams& P, const zxc_b200_job_t& job, u8* 
     }
 }
 
-template <bool UNITS, bool DEFERRED, bool HAS_DICT>
+/* LEAN: decode_job<LEAN>; each job it defers is marked D2_DEFER_STATUS and listed for a DEFERRED launch that follows.
+ * The lean instance runs at the general one's 7 CTAs per SM: at 8 (64 registers) and 10 (48) it spilled more and
+ * measured slower (DESIGN.md section 9). */
+template <bool UNITS, bool DEFERRED, bool HAS_DICT, bool LEAN>
 __global__ void __launch_bounds__(CTA_THREADS, CTAS_PER_SM) zxc_decode_kernel(const DecodeParams P) {
     extern __shared__ __align__(16) u8 smem[];
     const u32 lane = threadIdx.x & 31;
@@ -1126,6 +1145,7 @@ __global__ void __launch_bounds__(CTA_THREADS, CTAS_PER_SM) zxc_decode_kernel(co
 #endif
     if (DEFERRED) {
         const u32 n_def = *P.defer_count;
+        if (n_def == 0) return;
         if (n_def <= P.defer_cap) { /* the listed jobs, one per claim */
             for (;;) {
                 unsigned long long k = 0;
@@ -1134,7 +1154,7 @@ __global__ void __launch_bounds__(CTA_THREADS, CTAS_PER_SM) zxc_decode_kernel(co
                 if (k >= n_def) break;
                 const u32 j = P.defer_list[k];
                 const zxc_b200_job_t job = P.jobs[j];
-                const int r = decode_job<UNITS, HAS_DICT>(P, job, scratch, ring, lane);
+                const int r = decode_job<UNITS, HAS_DICT, false>(P, job, scratch, ring, lane);
                 flush_wait(lane); /* nothing of this block is still on its way out of the ring */
                 __syncwarp();
                 if (lane == 0) P.status[j] = r;
@@ -1153,7 +1173,7 @@ __global__ void __launch_bounds__(CTA_THREADS, CTAS_PER_SM) zxc_decode_kernel(co
                 const unsigned long long j = b + (u32)(__ffs(m) - 1);
                 m &= m - 1;
                 const zxc_b200_job_t job = P.jobs[j];
-                const int r = decode_job<UNITS, HAS_DICT>(P, job, scratch, ring, lane);
+                const int r = decode_job<UNITS, HAS_DICT, false>(P, job, scratch, ring, lane);
                 flush_wait(lane); /* nothing of this block is still on its way out of the ring */
                 __syncwarp();
                 if (lane == 0) P.status[j] = r;
@@ -1167,10 +1187,16 @@ __global__ void __launch_bounds__(CTA_THREADS, CTAS_PER_SM) zxc_decode_kernel(co
         j = __shfl_sync(FULL, j, 0);
         if (j >= P.n_jobs) break;
         const zxc_b200_job_t job = P.jobs[j];
-        const int r = decode_job<UNITS, HAS_DICT>(P, job, scratch, ring, lane);
-                flush_wait(lane); /* nothing of this block is still on its way out of the ring */
+        const int r = decode_job<UNITS, HAS_DICT, LEAN>(P, job, scratch, ring, lane);
+        flush_wait(lane); /* nothing of this block is still on its way out of the ring */
         __syncwarp();
-        if (lane == 0) P.status[j] = r;
+        if (lane == 0) {
+            P.status[j] = r;
+            if (LEAN && r == D2_DEFER_STATUS) {
+                const u32 slot = atomicAdd(P.defer_count, 1u);
+                if (slot < P.defer_cap) P.defer_list[slot] = (u32)j;
+            }
+        }
     }
 }
 

@@ -5,7 +5,9 @@
  *
  * Decode launches (launch_decode below):
  *   zxc_decode_kernel   (zxc_decode.cuh)  one warp per block, any block size / section encoding: every launch by
- *                       default (instances: sequence-centric or output-centric body, with / without dictionary)
+ *                       default (instances: sequence-centric or output-centric body, with / without dictionary);
+ *                       without checksum verification its lean instance runs first and the general one decodes
+ *                       what the lean one deferred (GHI blocks, Huffman sections)
  *   zxc_decode2_kernel  (zxc_decode2.cuh) one CTA per block of <= 64 KiB, window in shared memory, cp.async.bulk in
  *                       and out; only with ZXC_B200_DECODE_V2=1 (it measured 6.7x slower on the H100, DESIGN.md section 3c); what
  *                       it defers (entropy-coded sections, checksum verification) goes to zxc_decode_kernel
@@ -622,10 +624,10 @@ static size_t d2_spill_bytes(const D2Config* c) {
 extern "C" size_t zxc_b200_decode_scratch_size(uint32_t block_size) {
     if (zxg_init() != ZXC_OK) return 0;
     const size_t warps = (size_t)g_sm_count * CTAS_PER_SM * WARPS_PER_CTA;
-    size_t n = warps * scratch_stride_for(block_size);
+    size_t n = warps * scratch_stride_for(block_size) + 512; /* room to align the regions behind it to 256 bytes */
     D2Config c;
-    if (d2_config(block_size, &c)) n += d2_spill_bytes(&c) + 256 + (size_t)DEFER_CAP * 4 + 256;
-    return n + SCRATCH_TAIL;
+    if (d2_config(block_size, &c)) n += d2_spill_bytes(&c) + 256;
+    return n + (size_t)DEFER_CAP * 4 + SCRATCH_TAIL;
 }
 
 /* d_counter: two 64-bit work counters (zeroed here) */
@@ -662,13 +664,16 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
      * request (ZXC_B200_UNITS=1). */
     const bool units = (P.flags & FLAG_UNITS_ON) != 0;
     P.block_cap = block_size;
-    P.defer_list = NULL;
-    P.defer_count = NULL;
-    P.defer_cap = 0;
     const int grid = grid_for(n_jobs);
     const size_t warp_scratch = (size_t)grid * WARPS_PER_CTA * P.scratch_stride;
     if (warp_scratch > scratch_size) return ZXC_ERROR_MEMORY;
     if (cudaMemsetAsync(d_counter, 0, 3 * sizeof(unsigned long long), st) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    /* deferred-job list behind the per-warp scratch (and the block-cooperative kernel's spill area); its counter is the
+     * third work counter.  A scratch too small for it leaves the list empty: the second launch scans the status array. */
+    size_t off = (warp_scratch + 255) & ~(size_t)255;
+    P.defer_count = (u32*)(d_counter + 2);
+    P.defer_cap = off + (size_t)DEFER_CAP * 4 <= scratch_size ? DEFER_CAP : 0u;
+    P.defer_list = (u32*)((u8*)d_scratch + off);
     D2Config c;
     if (!verify && d2_config(block_size, &c)) {
         /* launch 1: one CTA per block, window in shared memory; launch 2: whatever it deferred */
@@ -695,19 +700,17 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
         Q.spill_stride = c.spill_stride;
         const u32 resident = (u32)(g_sm_count > 0 ? g_sm_count : 132) * c.ctas_per_sm;
         const u32 grid2 = n_jobs < resident ? n_jobs : resident;
-        size_t off = (warp_scratch + 255) & ~(size_t)255;
         if (c.spill_stride) {
             if (off + (size_t)grid2 * c.spill_stride * sizeof(z2_rec_t) > scratch_size) return ZXC_ERROR_MEMORY;
             Q.spill = (z2_rec_t*)((u8*)d_scratch + off);
             off = (off + d2_spill_bytes(&c) + 255) & ~(size_t)255;
         }
-        /* deferred-job list behind the spill area; its counter is the third work counter */
-        Q.defer_count = (u32*)(d_counter + 2);
-        Q.defer_cap = off + (size_t)DEFER_CAP * 4 <= scratch_size ? DEFER_CAP : 0u;
-        Q.defer_list = (u32*)((u8*)d_scratch + off);
-        P.defer_list = Q.defer_list;
-        P.defer_count = Q.defer_count;
-        P.defer_cap = Q.defer_cap;
+        /* the list moves behind the spill area */
+        P.defer_cap = off + (size_t)DEFER_CAP * 4 <= scratch_size ? DEFER_CAP : 0u;
+        P.defer_list = (u32*)((u8*)d_scratch + off);
+        Q.defer_count = P.defer_count;
+        Q.defer_cap = P.defer_cap;
+        Q.defer_list = P.defer_list;
         Q.trace = NULL;
         const int want_trace = getenv("ZXC_B200_D2_TRACE") != NULL; /* development: per-phase cycle counts */
         if (want_trace && cudaMalloc((void**)&Q.trace, (size_t)n_jobs * 128) == cudaSuccess)
@@ -749,15 +752,25 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
     }
     /* the dictionary-free instance carries neither the dictionary pointer nor its source classification (zxc_decode.cuh) */
     const bool has_dict = P.dict != NULL && P.dict_size != 0;
+    if (!verify && !units && !(P.flags & FLAG_DEFERRED)) {
+        /* launch 1: the lean instance decodes the RAW blocks and the GLO blocks without Huffman sections and lists the
+         * rest; launch 2 below: the general instance decodes the listed jobs (its warps exit at once when there are none) */
+        if (has_dict) zxc_decode_kernel<false, false, true, true><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+        else zxc_decode_kernel<false, false, false, true><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+        if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+        P.flags |= FLAG_DEFERRED;
+        P.counter = d_counter + 1;
+    }
     if (P.flags & FLAG_DEFERRED) {
-        if (has_dict) zxc_decode_kernel<false, true, true><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
-        else zxc_decode_kernel<false, true, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+        if (has_dict) zxc_decode_kernel<false, true, true, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+        else zxc_decode_kernel<false, true, false, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
     } else if (units) {
-        if (has_dict) zxc_decode_kernel<true, false, true><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
-        else zxc_decode_kernel<true, false, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+        if (has_dict) zxc_decode_kernel<true, false, true, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+        else zxc_decode_kernel<true, false, false, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
     } else {
-        if (has_dict) zxc_decode_kernel<false, false, true><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
-        else zxc_decode_kernel<false, false, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+        if (has_dict) zxc_decode_kernel<false, false, true, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+        else zxc_decode_kernel<false, false, false, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
     }
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
@@ -766,13 +779,10 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
 /* device scratch one launch over n_jobs blocks needs (without the counter tail) */
 static size_t launch_scratch_bytes(u32 n_jobs, u32 block_size) {
     size_t n = (size_t)grid_for(n_jobs) * WARPS_PER_CTA * scratch_stride_for(block_size);
+    n = (n + 255) & ~(size_t)255;
     D2Config c;
-    if (d2_config(block_size, &c)) {
-        n = (n + 255) & ~(size_t)255;
-        if (c.spill_stride) n = (n + d2_spill_bytes(&c) + 255) & ~(size_t)255;
-        n += (size_t)DEFER_CAP * 4 + 256;
-    }
-    return n;
+    if (d2_config(block_size, &c) && c.spill_stride) n = (n + d2_spill_bytes(&c) + 255) & ~(size_t)255;
+    return n + (size_t)DEFER_CAP * 4 + 256;
 }
 
 extern "C" int zxc_b200_decode_blocks(const void* d_src, void* d_dst, const zxc_b200_job_t* d_jobs,
