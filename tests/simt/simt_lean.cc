@@ -13,29 +13,10 @@ extern "C" { uint32_t simt_lean_deferred; /* jobs the lean instance left to the 
 extern "C" uint64_t simt_decode_two_stage(const u8* src, uint64_t src_size, u8* dst, uint64_t dst_size,
                                           const zxc_b200_job_t* jobs, u32 n_jobs, i32* status, const u8* dict,
                                           u32 dict_size, const u8* dict_huf, u32 block_cap, uint64_t seed, int* oob_writes) {
-    /* device buffers with a guard band either side: word loads may touch a few bytes outside, stores must not */
-    std::vector<u8> in(src_size + 2 * PAD, 0xA5), out(dst_size + 2 * PAD, 0x5A), dct((size_t)dict_size + 128 + 2 * PAD, 0x33);
-    memcpy(in.data() + PAD, src, src_size);
-    if (dict && dict_size) memcpy(dct.data() + PAD, dict, dict_size);
-    if (dict_huf) memcpy(dct.data() + PAD + dict_size, dict_huf, 128);
-    const u32 stride = scr_stride(block_cap);
-    std::vector<u8> scratch((size_t)stride + 2 * PAD, 0x77);
-    unsigned long long counter = 0;
-    DecodeParams P;
-    memset(&P, 0, sizeof P);
-    P.src = in.data() + PAD;
-    P.dst = out.data() + PAD;
-    P.jobs = jobs;
-    P.status = status;
-    P.dict = (dict && dict_size) ? dct.data() + PAD : nullptr;
-    P.dict_huf = dict_huf ? dct.data() + PAD + dict_size : nullptr;
-    P.scratch = scratch.data() + PAD;
-    P.counter = &counter;
-    P.n_jobs = n_jobs;
-    P.dict_size = dict_size;
-    P.scratch_stride = stride;
-    P.flags = 0;
-    P.block_cap = block_cap;
+    /* device buffers with a guard band either side (or guard pages): word loads may touch a few bytes outside, stores
+     * must not */
+    SimtDevice dev(src, src_size, dst_size, jobs, n_jobs, status, dict, dict_size, dict_huf, block_cap, 0);
+    const DecodeParams& P = dev.P;
     const bool has_dict = P.dict != nullptr && P.dict_size != 0;
     uint64_t rendezvous = 0;
     simt_lean_deferred = 0;
@@ -58,9 +39,7 @@ extern "C" uint64_t simt_decode_two_stage(const u8* src, uint64_t src_size, u8* 
             if (lean && status[j] == D2_DEFER_STATUS) simt_lean_deferred++;
         }
     }
-    int bad = 0;
-    for (u32 k = 0; k < PAD; k++) bad += (out[k] != 0x5A) + (out[PAD + dst_size + k] != 0x5A);
+    const int bad = dev.finish(dst);
     if (oob_writes) *oob_writes = bad;
-    memcpy(dst, out.data() + PAD, dst_size);
     return rendezvous;
 }

@@ -6,7 +6,6 @@ through the C ABI on the GPU, with and without a dictionary, and with more defer
 holds.  The emulator also runs the reference differential and the damaged-block parity along this route."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,28 +13,11 @@ import pytest
 import zxc_corpus as zc
 import zxc_ctypes as z
 import zxc_simt as zs
+from zxc_simt import lean_emu  # noqa: F401  (fixture)
 from test_oracle import CASES, G, make_case
 
 BLOCK_CAP = 65536
 DEFER_CAP = 1 << 16  # zxc_gpu.cu: deferred jobs the list holds; beyond that the general launch scans the status array
-
-
-@pytest.fixture(scope="module")
-def lean_emu(tmp_path_factory):
-    """tests/simt/simt_lean.cc built like tests/simt/Makefile builds the emulator, into a temporary directory"""
-    so = str(tmp_path_factory.mktemp("simt_lean") / "libzxc_simt_lean.so")
-    root = os.path.dirname(zs.HERE)
-    r = subprocess.run(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall", "-Wno-unknown-pragmas",
-                        "-Wno-unused-function", "-I.", "-I" + os.path.join(root, "include"),
-                        "-I" + os.path.join(root, "zxc_b200", "csrc"), "-o", so, "simt_lean.cc", "simt_rt.cc"],
-                       cwd=zs.SIMT_DIR, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0, r.stdout[-3000:]
-    lib = C.CDLL(so)
-    lib.simt_decode_two_stage.restype = C.c_uint64
-    lib.simt_decode_two_stage.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32,
-                                          C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint64,
-                                          C.c_void_p]
-    return lib
 
 
 def plan_frame(prod, fb):

@@ -112,7 +112,7 @@ def test_kernel_source_with_bulk_copy_staging():
     cp.async.bulk, ring flushed by bulk stores: -DZXC_STAGE=1 -DZXC_STAGE_LIT=1 -DZXC_BULK_FLUSH=1) through the same
     tests.  The emulator performs a bulk load when it is issued and a bulk store only when it is waited for, and keeps
     the mbarriers' books: one copy in flight per barrier, every wait on the parity it names, nothing in flight at
-    the end of a block."""
+    the end of a block.  The synthetic-sequence catalogue (test_blockgen_decode.py) runs in the same flavour."""
     import subprocess
     import sys
     here = os.path.dirname(os.path.abspath(__file__))
@@ -120,7 +120,8 @@ def test_kernel_source_with_bulk_copy_staging():
     r = subprocess.run(["make", "-s", "SO=" + so, "EXTRA=-DZXC_STAGE=1 -DZXC_STAGE_LIT=1 -DZXC_BULK_FLUSH=1"],
                        cwd=os.path.join(here, "simt"), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     assert r.returncode == 0, r.stdout
-    env = dict(os.environ, ZXC_SIMT_SO=so)
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-x", "-q", "-p", "no:cacheprovider"],
+    env = dict(os.environ, ZXC_SIMT_SO=so, ZXC_SIMT_EXTRA="-DZXC_STAGE=1 -DZXC_STAGE_LIT=1 -DZXC_BULK_FLUSH=1")
+    r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), os.path.join(here, "test_blockgen_decode.py"),
+                        "-x", "-q", "-p", "no:cacheprovider", "-m", "not gpu"],
                        env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=1200)
     assert r.returncode == 0, r.stdout[-2000:]

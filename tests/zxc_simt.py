@@ -6,6 +6,7 @@ import os
 import subprocess
 
 import numpy as np
+import pytest
 
 import zxc_ctypes as z
 
@@ -69,3 +70,23 @@ def decode_frame(prod, frame, dict=None, dict_huf=None, verify=0, units=0, seed=
                                   h.ctypes.data if h is not None else None, max(info.block_size, 4096),
                                   1 if (verify and info.has_checksum) else 0, units, seed, C.byref(oob))
     return list(status)[:nb], out[:total], oob.value, rv
+
+
+@pytest.fixture(scope="session")
+def lean_emu(tmp_path_factory):
+    """tests/simt/simt_lean.cc -- the two-launch route: lean instance, then the general one for what it deferred --
+    built like tests/simt/Makefile builds the emulator, into a temporary directory"""
+    so = str(tmp_path_factory.mktemp("simt_lean") / "libzxc_simt_lean.so")
+    root = os.path.dirname(HERE)
+    extra = os.environ.get("ZXC_SIMT_EXTRA", "").split()  # the flavour of a variant build (ZXC_SIMT_SO)
+    r = subprocess.run(["g++", *extra, "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall", "-Wno-unknown-pragmas",
+                        "-Wno-unused-function", "-I.", "-I" + os.path.join(root, "include"),
+                        "-I" + os.path.join(root, "zxc_b200", "csrc"), "-o", so, "simt_lean.cc", "simt_rt.cc"],
+                       cwd=SIMT_DIR, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    assert r.returncode == 0, r.stdout[-3000:]
+    lib = C.CDLL(so)
+    lib.simt_decode_two_stage.restype = C.c_uint64
+    lib.simt_decode_two_stage.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32,
+                                          C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint64,
+                                          C.c_void_p]
+    return lib

@@ -492,6 +492,7 @@ __device__ __forceinline__ void flush_wait(u32 lane) {
 /* whole-warp match copy of n bytes into the ring at d from distance off */
 __device__ __forceinline__ void warp_match_to_ring(const Window& w, u32 d, u32 off, u32 n, u32 lane) {
     const u32 mask = RING_BYTES - 1;
+    ZXC_STAT(16, d < off); /* byte copies that start in the dictionary */
     if (off >= 32) {
         /* chunk c only reads bytes below its own start: earlier chunks are complete */
         for (u32 c = 0; c < n; c += 32) {
@@ -503,6 +504,7 @@ __device__ __forceinline__ void warp_match_to_ring(const Window& w, u32 d, u32 o
         /* period-`off` replication of the complete window [d-off, d): lane r holds window byte r, byte k of the match
          * is window byte k mod off -- fetched by shuffle, the residue stepped by 32 mod off (no division per byte) */
         const u32 mine = lane < off ? (u32)window_byte(w, (i32)d - (i32)off + (i32)lane) : 0u;
+        ZXC_STAT(15, 1); /* period replications */
 #if ZXC_FASTMOD
         /* x mod off for x <= 32, off < 32 without the integer division: with a reciprocal good to a few ulp the float
          * quotient is at most one too small at exact multiples and never too large (between multiples the true quotient
@@ -894,6 +896,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             /* ---- giant sequence (lane 0): bypass the ring, global -> global ---- */
             const u32 g_ll = __shfl_sync(FULL, ll, 0), g_ml = __shfl_sync(FULL, ml, 0),
                       g_off = __shfl_sync(FULL, off, 0);
+            ZXC_STAT(9, 1); /* giant sequences */
             if (L + g_ll > n_lit_avail || (u64)O + g_ll + g_ml > cap) {
                 ST_CLOSE();
                 return ZXC_ERROR_OVERFLOW;
@@ -925,12 +928,15 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             continue;
         }
 
+        ZXC_STAT(10, m < nvalid);              /* partial batches */
+        ZXC_STAT(11, m < nvalid && !use_vals); /* ... that re-walk the varint cursor */
         /* ---- validation ---- */
         const bool act = lane < m;
         const bool ovf = act && (lit_start + ll > n_lit_avail || out_start + tot > cap);
         const bool bad = act && (mdst + dict_size < off);
         const u32 m_err = __ballot_sync(FULL, ovf || bad);
         if (ZXC_RARE(m_err != 0)) {
+            ZXC_STAT(19, 1); /* verdicts raised by a batch */
             const int code = ovf ? ZXC_ERROR_OVERFLOW : ZXC_ERROR_BAD_OFFSET;
             ST_CLOSE();
             return __shfl_sync(FULL, code, __ffs(m_err) - 1);
@@ -1014,6 +1020,10 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             ZXC_STAT(5, m_grp != 0);                                  /* long-copy calls */
             ZXC_STAT(6, __popc(__ballot_sync(FULL, ready && !lok && !gok))); /* slow items */
             ZXC_STAT(7, __ballot_sync(FULL, ready && lok) != 0);      /* passes with a per-lane item */
+            ZXC_STAT(17, __popc(__ballot_sync(FULL, !lit_pass && ready && (lok || gok) && src_lo < 0)));  /* dictionary words */
+            ZXC_STAT(18, __popc(__ballot_sync(FULL, !lit_pass && ready && !lok && !gok)));  /* match byte path */
+            ZXC_STAT(20, __popc(__ballot_sync(FULL, !lit_pass && ready && (lok || gok) && near))); /* ring words */
+            ZXC_STAT(21, __popc(__ballot_sync(FULL, !lit_pass && ready && (lok || gok) && !near && src_lo >= 0))); /* global words */
             if (m_grp) balanced_copy_words(ring_s, m_grp, it_d, it_sp, it_n, lane);
             u32 m_slow = __ballot_sync(FULL, ready && !lok && !gok);
             while (ZXC_RARE(m_slow != 0)) { /* ring wrap, close overlap, dictionary, straddling sources: byte paths */
