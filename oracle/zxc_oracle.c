@@ -340,6 +340,7 @@ static size_t popcount_prefix(const uint8_t* bits, size_t nbits) {
 
 /* payload excludes the 128-byte lengths header */
 static int huf_decode_runs(htree_t* t, const uint8_t* payload, size_t psize, uint8_t* out, size_t n) {
+    if (n == 0) return ZXO_E_CORRUPT_DATA; /* zxc_pivco_decode_core rejects an empty section (zxc_huffman.c:2276) */
     /* pass 1: walk the BFS order, assign runs and counts (zxc_huffman.c:2297-2328) */
     const uint8_t* p = payload;
     const uint8_t* const pend = payload + psize;
@@ -378,16 +379,19 @@ static int huf_decode_runs(htree_t* t, const uint8_t* payload, size_t psize, uin
                 return ZXO_E_CORRUPT_DATA;
         }
     }
-    /* pass 2: per-symbol top-down walk with rank queries */
+    /* pass 2: per-symbol top-down walk; a node's run is read in order by the symbols that pass through it, so the
+     * index of a symbol at a node is the number that passed before it */
+    size_t* seen = (size_t*)calloc((size_t)t->n_nodes, sizeof(size_t));
+    if (!seen) return ZXO_E_MEMORY;
     for (size_t k = 0; k < n; k++) {
         int id = 0;
-        size_t idx = k;
         for (;;) {
             const hnode_t* nd = &t->n[id];
             if (nd->sym >= 0) {
                 out[k] = (uint8_t)nd->sym;
                 break;
             }
+            const size_t idx = seen[id]++;
             if (nd->flat_d) {
                 const size_t bitpos = idx * (size_t)nd->flat_d;
                 int cur = id;
@@ -400,17 +404,14 @@ static int huf_decode_runs(htree_t* t, const uint8_t* payload, size_t psize, uin
                 break;
             }
             const int bit = (nd->run[idx >> 3] >> (idx & 7)) & 1;
-            const size_t ones_before = popcount_prefix(nd->run, idx);
-            if (bit) {
-                id = nd->right;
-                idx = ones_before;
-            } else {
-                id = nd->left;
-                idx = idx - ones_before;
+            id = bit ? nd->right : nd->left;
+            if (id < 0) {
+                free(seen);
+                return ZXO_E_CORRUPT_DATA;
             }
-            if (id < 0) return ZXO_E_CORRUPT_DATA;
         }
     }
+    free(seen);
     return ZXO_OK;
 }
 
@@ -479,8 +480,10 @@ static int lz_finish(lz_t* z) {
 }
 
 /* GLO payload (zxc_decompress.c:847-1209, zxc_common.c:773-795) */
+/* block_size: the frame's block size, the reference's chunk_size; its token buffer holds block_size / 5 + 16 sequences
+ * (zxc_common.c:142-156, zxc_decompress.c:801) */
 static int decode_glo(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, const uint8_t* dict,
-                      size_t dict_size, const uint8_t* dict_huf) {
+                      size_t dict_size, const uint8_t* dict_huf, size_t block_size) {
     if (n < SUB_HDR) return ZXO_E_BAD_HEADER;
     const uint32_t n_seq = le32(src), n_lit = le32(src + 4);
     const uint8_t enc_lit = src[8], enc_tok = src[9], enc_off = src[11];
@@ -509,6 +512,7 @@ static int decode_glo(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, co
         } else {
             if (n_lit > cap) return ZXO_E_DST_TOO_SMALL;
             if (enc_lit == 3 && !dict_huf) return ZXO_E_DICT_REQUIRED;
+            if (n_lit > block_size) return ZXO_E_CORRUPT_DATA; /* lit_buffer_cap (:774) */
             lit_buf = (uint8_t*)malloc((size_t)n_lit + 1);
             if (!lit_buf) return ZXO_E_MEMORY;
             rc = huf_decode_section(p_data, lit_comp, enc_lit == 3 ? dict_huf : NULL, lit_buf, n_lit);
@@ -518,6 +522,7 @@ static int decode_glo(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, co
     } else if (enc_lit == 1) { /* :906-978 */
         if (n_lit > 0) {
             if (n_lit > cap) return ZXO_E_DST_TOO_SMALL;
+            if (n_lit > block_size) return ZXO_E_CORRUPT_DATA; /* lit_buffer_cap (:914) */
             if (lit_comp > avail) return ZXO_E_CORRUPT_DATA;
             lit_buf = (uint8_t*)malloc((size_t)n_lit + 1);
             if (!lit_buf) return ZXO_E_MEMORY;
@@ -549,6 +554,10 @@ static int decode_glo(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, co
         const uint8_t* ext = offs + sz_off;
         const uint8_t* const ext_end = p_data + avail;
         if (enc_tok == 2) { /* :1019-1022 */
+            if ((size_t)n_seq > block_size / MIN_MATCH + 16) {
+                rc = ZXO_E_CORRUPT_DATA;
+                goto done;
+            }
             tok_buf = (uint8_t*)malloc((size_t)n_seq + 1);
             if (!tok_buf) {
                 rc = ZXO_E_MEMORY;
@@ -609,9 +618,9 @@ static int decode_ghi(const uint8_t* src, size_t n, uint8_t* dst, size_t cap, co
 }
 
 /* zxc_decompress_chunk_wrapper_body (zxc_decompress.c:1646-1695) */
-int zxo_decode_block(const uint8_t* blk, size_t blk_size, uint8_t* dst, size_t dst_cap,
-                     const uint8_t* dict, size_t dict_size, const uint8_t* dict_huf,
-                     int verify_checksum) {
+int zxo_decode_block_bs(const uint8_t* blk, size_t blk_size, uint8_t* dst, size_t dst_cap,
+                        const uint8_t* dict, size_t dict_size, const uint8_t* dict_huf,
+                        int verify_checksum, size_t block_size) {
     if (blk_size < BLK_HDR) return ZXO_E_SRC_TOO_SMALL;
     const uint8_t type = blk[0];
     const uint32_t comp = le32(blk + 3);
@@ -621,7 +630,7 @@ int zxo_decode_block(const uint8_t* blk, size_t blk_size, uint8_t* dst, size_t d
     if (verify_checksum && le32(data + comp) != zxo_checksum(data, comp)) return ZXO_E_BAD_CHECKSUM;
     switch (type) {
         case BT_GLO:
-            return decode_glo(data, comp, dst, dst_cap, dict, dict_size, dict_huf);
+            return decode_glo(data, comp, dst, dst_cap, dict, dict_size, dict_huf, block_size);
         case BT_GHI:
             return decode_ghi(data, comp, dst, dst_cap, dict, dict_size);
         case BT_RAW:
@@ -633,6 +642,16 @@ int zxo_decode_block(const uint8_t* blk, size_t blk_size, uint8_t* dst, size_t d
         default:
             return ZXO_E_BAD_BLOCK_TYPE;
     }
+}
+
+/* the block API (zxc_decompress_block, zxc_dispatch.c:1742): the block size is dst_cap rounded up to a power of two,
+ * at least the smallest block size */
+int zxo_decode_block(const uint8_t* blk, size_t blk_size, uint8_t* dst, size_t dst_cap,
+                     const uint8_t* dict, size_t dict_size, const uint8_t* dict_huf,
+                     int verify_checksum) {
+    size_t bs = (size_t)1 << 12;
+    while (bs < dst_cap) bs <<= 1;
+    return zxo_decode_block_bs(blk, blk_size, dst, dst_cap, dict, dict_size, dict_huf, verify_checksum, bs);
 }
 
 /* zxc_read_file_header (zxc_common.c:574-603) */
@@ -678,6 +697,19 @@ int64_t zxo_decompress(const uint8_t* src, size_t src_size, uint8_t* dst, size_t
         if (!dict || dict_size == 0) return ZXO_E_DICT_REQUIRED;
         if (zxo_dict_id(dict, dict_size, dict_huf) != did) return ZXO_E_DICT_MISMATCH;
     }
+    if (dict_size && dict_huf) { /* zxc_cctx_attach_dict_huf (zxc_common.c:490-512) */
+        int any = 0;
+        for (int i = 0; i < 128; i++) any |= dict_huf[i];
+        if (!any) {
+            dict_huf = NULL; /* an all-zero table is no table */
+        } else {
+            htree_t* t = (htree_t*)malloc(sizeof(htree_t));
+            if (!t) return ZXO_E_MEMORY;
+            const int brc = huf_build(t, dict_huf);
+            free(t);
+            if (brc != ZXO_OK) return ZXO_E_CORRUPT_DATA;
+        }
+    }
     const int verify = file_cks && checksum_enabled;
     const size_t work_sz = bs + TAIL_PAD;
     uint8_t* work = (uint8_t*)malloc(work_sz);
@@ -716,7 +748,7 @@ int64_t zxo_decompress(const uint8_t* src, size_t src_size, uint8_t* dst, size_t
             ret = (int64_t)op;
             break;
         }
-        const int res = zxo_decode_block(ip, rem, work, work_sz, dict, dict_size, dict_huf, verify);
+        const int res = zxo_decode_block_bs(ip, rem, work, work_sz, dict, dict_size, dict_huf, verify, bs);
         if (res < 0) {
             ret = res;
             break;

@@ -50,7 +50,12 @@ uint32_t zxo_dict_id(const void* dict, size_t dict_size, const void* huf128);
 
 /* One on-disk block (8-byte header + payload [+4 checksum if has_checksum]).
  * Returns decoded bytes or a negative code.  `dict` (may be NULL) is the
- * window prefix matches may reach into.  src/lib/zxc_decompress.c:1646-1695. */
+ * window prefix matches may reach into.  src/lib/zxc_decompress.c:1646-1695.
+ * `block_size` is the frame's block size, which bounds the Huffman-coded token count; zxo_decode_block takes it from
+ * dst_cap rounded up to a block size, as the block API zxc_decompress_block does. */
+int zxo_decode_block_bs(const uint8_t* blk, size_t blk_size, uint8_t* dst, size_t dst_cap,
+                        const uint8_t* dict, size_t dict_size, const uint8_t* dict_huf,
+                        int verify_checksum, size_t block_size);
 int zxo_decode_block(const uint8_t* blk, size_t blk_size, uint8_t* dst, size_t dst_cap,
                      const uint8_t* dict, size_t dict_size, const uint8_t* dict_huf,
                      int verify_checksum);

@@ -21,7 +21,7 @@
 
 #include <vector>
 
-extern "C" { uint64_t simt_stat[32]; }
+extern "C" { uint64_t simt_stat[64]; }
 #define ZXC_STAT(i, v) do { const uint64_t zv_ = (uint64_t)(v); if (simt::g_warp->current == 0) simt_stat[i] += zv_; } while (0)
 
 #include <stdio.h>

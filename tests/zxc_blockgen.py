@@ -10,7 +10,12 @@ their source and destination offsets.
 
 Every block carries what it is meant to decode to, computed here by a plain byte loop over the sequences (the
 reference's lz_emit semantics, dictionary reads included): the decoded bytes, or the error code of the first sequence
-that cannot be emitted.  Huffman sections are not written; reference-encoded frames cover them.
+that cannot be emitted.
+
+GLO literal and token sections may also be PivCo Huffman sections (docs/FORMAT.md, PivCo): a 128-byte table of code
+lengths, then one run per emitting tree node in BFS order.  pivco_runs() writes them from 256 code lengths and a symbol
+string; pivco_decode() reads them back by walking the explicit code tree one branch at a time, with no rank tables.
+A caller may also hand in the table and the run bytes as they are, to build malformed sections.
 
 The header hashes and block checksums come from the test oracle (oracle/libzxc_oracle.so)."""
 import struct
@@ -20,6 +25,8 @@ import numpy as np
 MIN_MATCH = 5
 SLACK = 32
 OVERFLOW, BAD_OFFSET = -10, -9
+DST_TOO_SMALL, CORRUPT, DICT_REQUIRED = -2, -8, -15
+HUF_MAXLEN = 11
 
 _orc = None
 
@@ -143,14 +150,214 @@ def _escapes(seqs, esc):
     return bytes(ext), ended
 
 
+# ------------------------------------------------------------------------------------------------------------------
+# PivCo sections
+# ------------------------------------------------------------------------------------------------------------------
+def pack_lengths(lens):
+    """the 128-byte table: symbol 2i in the low nibble of byte i, 2i + 1 in the high one"""
+    lens = list(lens) + [0] * (256 - len(lens))
+    assert all(0 <= v <= 15 for v in lens)
+    return bytes(lens[2 * i] | (lens[2 * i + 1] << 4) for i in range(128))
+
+
+def unpack_lengths(table):
+    return [(table[s >> 1] >> (4 * (s & 1))) & 15 for s in range(256)]
+
+
+class PivcoTree:
+    """The explicit canonical code tree of 256 code lengths.  A node is (depth, prefix); `kind[node]` is "leaf",
+    "bitmap", a flat-root depth D >= 2 (every leaf below it sits D levels down) or "covered" (below a flat root).
+    `error` is set, and nothing else, when the lengths do not make a code the format accepts."""
+
+    def __init__(self, lens):
+        self.lens = list(lens)
+        self.error = None
+        present = [s for s in range(256) if self.lens[s]]
+        if any(v > HUF_MAXLEN for v in self.lens) or not present:
+            self.error = CORRUPT
+            return
+        kraft = sum(1 << (HUF_MAXLEN - self.lens[s]) for s in present)
+        self.single = len(present) == 1 and self.lens[present[0]] == 1
+        if kraft != 1 << HUF_MAXLEN and not self.single:
+            self.error = CORRUPT
+            return
+        self.code = [0] * 256
+        code = 0
+        prev = 0
+        for s in sorted(present, key=lambda s: (self.lens[s], s)):  # canonical: by (length, symbol)
+            code <<= self.lens[s] - prev
+            prev = self.lens[s]
+            self.code[s] = code
+            code += 1
+        self.leaf = {(self.lens[s], self.code[s]): s for s in present}
+        internal = set()
+        for d, c in self.leaf:
+            for k in range(d):
+                internal.add((k, c >> (d - k)))
+        self.internal = internal
+        self.kind = {}
+        for node in sorted(internal | set(self.leaf)):  # BFS: by depth, then prefix
+            d, v = node
+            if node in self.leaf:
+                self.kind[node] = "leaf"
+            if d and self.kind.get((d - 1, v >> 1)) in ("covered",) + tuple(range(2, HUF_MAXLEN + 1)):
+                self.kind[node] = "covered"
+            elif node in internal:
+                u = self._uniform(node)
+                self.kind[node] = u if u >= 2 else "bitmap"
+        self.bfs = sorted(internal | set(self.leaf))
+
+    def _uniform(self, node):
+        d, v = node
+        if node in self.leaf:
+            return 0
+        kids = [(d + 1, 2 * v), (d + 1, 2 * v + 1)]
+        if any(k not in self.leaf and k not in self.internal for k in kids):
+            return -1
+        a, b = self._uniform(kids[0]), self._uniform(kids[1])
+        return a + 1 if a == b and a >= 0 else -1
+
+    def emitting(self):
+        return [n for n in self.bfs if self.kind[n] not in ("leaf", "covered")]
+
+    def flat_depths(self):
+        return sorted({self.kind[n] for n in self.emitting() if self.kind[n] != "bitmap"})
+
+
+def _group(keys, nodes):
+    """for each node value in `nodes`: the positions of `keys` equal to it, in order"""
+    order = np.argsort(keys, kind="stable")
+    sk = keys[order]
+    lo = np.searchsorted(sk, nodes, "left")
+    hi = np.searchsorted(sk, nodes, "right")
+    return [order[a:b] for a, b in zip(lo, hi)]
+
+
+def pivco_runs(lens, syms, sizes=None):
+    """the run area of `syms` under the code of `lens`, node by node in BFS order: a bitmap node writes one bit per
+    symbol through it (1 = right), a flat root of depth D the symbol's D-bit path (first step in bit 0), both packed
+    LSB-first; leaves and covered nodes write nothing.  `sizes`, a list, receives (node, kind, count, bytes) per run."""
+    t = PivcoTree(lens)
+    assert t.error is None, "the lengths do not make a code"
+    syms = np.frombuffer(bytes(syms), np.uint8)
+    assert all(t.lens[s] for s in set(syms.tolist())), "a symbol without a code"
+    L = np.array(t.lens, np.int64)[syms]
+    Cd = np.array(t.code, np.int64)[syms]
+    out = bytearray()
+    emit = t.emitting()
+    for d in range(HUF_MAXLEN + 1):
+        level = [n for n in emit if n[0] == d]
+        if not level:
+            continue
+        act = np.nonzero(L > d)[0]
+        groups = _group(Cd[act] >> (L[act] - d), np.array([v for _, v in level], np.int64))
+        for (_, v), g in zip(level, groups):
+            idx = act[g]
+            kind = t.kind[(d, v)]
+            if kind == "bitmap":
+                bits = (Cd[idx] >> (L[idx] - d - 1)) & 1
+            else:
+                bits = np.stack([(Cd[idx] >> (L[idx] - d - 1 - j)) & 1 for j in range(kind)], 1).reshape(-1)
+            run = np.packbits(bits.astype(np.uint8), bitorder="little").tobytes()
+            if sizes is not None:
+                sizes.append(((d, v), kind, idx.size, len(run)))
+            out += run
+    return bytes(out)
+
+
+def pivco_section(lens, syms):
+    """the whole section: the 128-byte table, then the runs"""
+    return pack_lengths(lens) + pivco_runs(lens, syms)
+
+
+def pivco_decode(table, runs, n):
+    """(status, bytes) of n symbols read from `runs` under the 128-byte `table`: the explicit tree walked one branch at
+    a time, every node's run consumed in order by the symbols that pass through it.  Verdicts are the reference's:
+    CORRUPT for a bad table, an empty section, a run area too short, or a symbol routed to a missing child."""
+    t = PivcoTree(unpack_lengths(table))
+    if t.error is not None or n == 0:
+        return CORRUPT, b""
+    runs = np.frombuffer(bytes(runs), np.uint8)
+    out = np.zeros(n, np.uint8)
+    at = np.zeros(n, np.int64)  # prefix of the node each unresolved symbol sits at
+    live = np.arange(n)
+    pos = 0
+    for d in range(HUF_MAXLEN + 1):
+        level = [nd for nd in t.emitting() if nd[0] == d]
+        if not level or not live.size:
+            continue
+        groups = _group(at[live], np.array([v for _, v in level], np.int64))
+        nxt = []
+        for (_, v), g in zip(level, groups):
+            idx = live[g]
+            c = idx.size
+            kind = t.kind[(d, v)]
+            nbytes = (c * (1 if kind == "bitmap" else kind) + 7) >> 3
+            if runs.size - pos < nbytes:
+                return CORRUPT, b""
+            bits = np.unpackbits(runs[pos:pos + nbytes], bitorder="little").astype(np.int64)
+            pos += nbytes
+            if kind == "bitmap":
+                b = bits[:c]
+                for bit in (0, 1):
+                    child = (d + 1, 2 * v + bit)
+                    sel = idx[b == bit]
+                    if child in t.leaf:
+                        out[sel] = t.leaf[child]
+                    elif child in t.internal:
+                        at[sel] = child[1]
+                        nxt.append(sel)
+                    elif sel.size:
+                        return CORRUPT, b""
+            else:
+                paths = bits[:c * kind].reshape(c, kind)
+                leafv = v
+                for j in range(kind):
+                    leafv = (leafv << 1) | paths[:, j]
+                lut = np.array([t.leaf.get((d + kind, x), 0) for x in range(v << kind, (v + 1) << kind)], np.uint8)
+                out[idx] = lut[leafv - (v << kind)]
+        live = np.sort(np.concatenate(nxt)) if nxt else np.zeros(0, np.int64)
+    return n, out.tobytes()
+
+
+class Huf:
+    """How a GLO section is Huffman-coded.  `lens`: 256 code lengths (the writer builds the runs); `table`: 128 table
+    bytes as they are (default: packed `lens`); `runs`: run bytes as they are (default: written from the symbols);
+    `extra`: bytes after the runs inside the section; `comp`: the section size the header declares (default: its
+    length)."""
+
+    def __init__(self, lens=None, table=None, runs=None, extra=b"", comp=None):
+        self.lens, self.table, self.runs, self.extra, self.comp = lens, table, runs, bytes(extra), comp
+
+    def section(self, syms, with_table=True, written=None):
+        """(section bytes, table, run area); `written` receives (lengths, symbols, table + runs) when the writer made
+        the whole section from the lengths"""
+        table = self.table if self.table is not None else pack_lengths(self.lens)
+        runs = self.runs if self.runs is not None else pivco_runs(self.lens, syms)
+        if written is not None and self.table is None and self.runs is None and not self.extra and self.comp is None:
+            written.append((self.lens, bytes(syms), table + runs))
+        sec = (table if with_table else b"") + runs + self.extra
+        return sec, table, runs + self.extra
+
+
 class Block:
     """A GLO or GHI block: `raw` is the on-disk block (8-byte header + payload [+ checksum]), `want` the status and
-    bytes it decodes to with `dict_bytes` into `cap` bytes."""
+    bytes it decodes to with `dict_bytes` into `cap` bytes.
+
+    GLO literals may be Huffman-coded (enc_lit = 2 with `lit_huf`, a Huf; enc_lit = 3 with the table `dict_huf` that
+    comes with the dictionary, and `lit_huf` giving its lengths or runs) and so may the tokens (enc_tok = 2 with
+    `tok_huf`).  `block_size` is the frame's block size: it bounds the Huffman-coded token count (block_size / 5 + 16,
+    the reference's token buffer) and the decoded literal count."""
 
     def __init__(self, seqs, tail=b"", kind="glo", enc_off=0, enc_lit=0, rle_plan=None, dict_bytes=b"", cap=None,
-                 extra_pad=0, checksum=False, n_lit=None):
+                 extra_pad=0, checksum=False, n_lit=None, lit_huf=None, tok_huf=None, dict_huf=None, block_size=None,
+                 n_seq=None):
         self.seqs, self.tail, self.kind = list(seqs), bytes(tail), kind
         self.dict_bytes = bytes(dict_bytes)
+        self.dict_huf = dict_huf
+        self.written_sections = []  # (lengths, symbols, table + runs) of the sections the writer made
+        self.decoded = []  # (lengths, symbols) of the sections that decode
+        self.pivco_verdict = False  # the verdict is the section decoder's
         lits = b"".join(s.lit for s in self.seqs) + self.tail
         n_lit_decl = len(lits) if n_lit is None else n_lit
         lits = (lits + bytes(max(0, n_lit_decl - len(lits))))[:n_lit_decl]  # a section holds what the header declares
@@ -162,13 +369,24 @@ class Block:
         if kind == "glo":
             tok = bytes((min(len(s.lit), 15) << 4) | min(s.ml - MIN_MATCH, 15) for s in self.seqs)
             offs = b"".join(bytes([s.off - 1]) if enc_off else struct.pack("<H", s.off - 1) for s in self.seqs)
+            lit_runs = tok_runs = None
             if enc_lit == 1:
                 lsec, self.rle_plan = rle_encode(lits, rle_plan)
                 desc = struct.pack("<I", len(lsec))
+            elif enc_lit in (2, 3):
+                lsec, _, lit_runs = lit_huf.section(lits, with_table=enc_lit == 2, written=self.written_sections)
+                desc = struct.pack("<I", len(lsec) if lit_huf.comp is None else lit_huf.comp)
             else:
                 lsec, desc = lits, b""
+            enc_tok = 0
+            if tok_huf is not None:
+                enc_tok = 2
+                tsec, tok_table, tok_runs = tok_huf.section(tok, written=self.written_sections)
+                desc += struct.pack("<I", len(tsec) if tok_huf.comp is None else tok_huf.comp)
+                tok = tsec
             body = tok + offs + ext
-            hdr = struct.pack("<IIBBBB", len(self.seqs), n_lit_decl, enc_lit, 0, 0, enc_off) + desc
+            hdr = struct.pack("<IIBBBB", len(self.seqs) if n_seq is None else n_seq, n_lit_decl, enc_lit, enc_tok, 0,
+                              enc_off) + desc
         else:
             words = b"".join(struct.pack("<I", (min(len(s.lit), 255) << 24) | (min(s.ml - MIN_MATCH, 255) << 16) | (s.off - 1))
                              for s in self.seqs)
@@ -181,9 +399,59 @@ class Block:
         out_len = len(lits) + sum(s.ml for s in self.seqs)
         if self.cap is None:
             self.cap = out_len
-        self.status, self.want = lz_decode(self.seqs, self.tail, self.cap, self.dict_bytes, n_lit_decl, lits)
+        self.block_size = block_size or max(4096, 1 << (max(self.cap, 1) - 1).bit_length())
+        self.status, self.want = None, b""
+        if kind == "glo" and (enc_lit >= 2 or enc_tok == 2):
+            self.status = self._huf_verdict(enc_lit, enc_tok, n_lit_decl, lits, lit_huf, tok_huf, lit_runs, tok_runs,
+                                            len(hdr), len(lsec), tok_huf and len(tok), n_seq)
+        if self.status is None:
+            self.status, self.want = lz_decode(self.seqs, self.tail, self.cap, self.dict_bytes, n_lit_decl, lits)
         self.checksum = checksum
         self.raw = block_bytes(1 if kind == "glo" else 2, self.payload, checksum)
+
+
+    def _huf_verdict(self, enc_lit, enc_tok, n_lit, lits, lit_huf, tok_huf, lit_runs, tok_runs, hdr_len, lsec_len,
+                     tsec_len, n_seq):
+        """the reference's section checks in its order (zxc_decompress.c:859-1023): a verdict, or None when the
+        sections decode to the literals and tokens the sequences say"""
+        avail = len(self.payload) - hdr_len
+        n_seq = len(self.seqs) if n_seq is None else n_seq
+        lit_comp = lsec_len if enc_lit < 2 or lit_huf.comp is None else lit_huf.comp
+        if enc_lit >= 2:
+            if lit_comp > avail:
+                return CORRUPT
+            if n_lit:
+                if n_lit > self.cap:
+                    return DST_TOO_SMALL
+                if enc_lit == 3 and self.dict_huf is None:
+                    return DICT_REQUIRED
+                if n_lit > self.block_size:
+                    return CORRUPT
+                if enc_lit == 2 and lit_comp < 128:
+                    return CORRUPT
+                # a section declared shorter than written ends where the header says
+                table = self.dict_huf if enc_lit == 3 else self.payload[hdr_len:hdr_len + 128]
+                rlen = lit_comp - (128 if enc_lit == 2 else 0)
+                st, got = pivco_decode(table, lit_runs[:rlen], n_lit)
+                if st < 0:
+                    self.pivco_verdict = True
+                    return st
+                self.decoded.append((unpack_lengths(table), got))
+                assert got == lits, "a malformed literal run that still decodes: give the case its own expectation"
+        tok_comp = n_seq if enc_tok != 2 else (tsec_len if tok_huf.comp is None else tok_huf.comp)
+        if lit_comp + tok_comp + n_seq * (1 if self.payload[11] else 2) > avail or avail - lit_comp < SLACK:
+            return CORRUPT
+        if enc_tok == 2:
+            if n_seq == 0 or n_seq > self.block_size // MIN_MATCH + 16 or tok_comp < 128:
+                return CORRUPT
+            table = self.payload[hdr_len + lit_comp:hdr_len + lit_comp + 128]
+            st, got = pivco_decode(table, tok_runs[:tok_comp - 128], n_seq)
+            if st < 0:
+                self.pivco_verdict = True
+                return st
+            self.decoded.append((unpack_lengths(table), got))
+            assert got[:len(self.seqs)] == bytes((min(len(s.lit), 15) << 4) | min(s.ml - MIN_MATCH, 15) for s in self.seqs)
+        return None
 
 
 def block_bytes(btype, payload, checksum):

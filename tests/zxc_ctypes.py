@@ -167,6 +167,8 @@ class Oracle:
         L.zxo_decode_block.restype = C.c_int
         L.zxo_decode_block.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                        C.c_size_t, C.c_void_p, C.c_int]
+        L.zxo_decode_block_bs.restype = C.c_int
+        L.zxo_decode_block_bs.argtypes = L.zxo_decode_block.argtypes + [C.c_size_t]
         L.zxo_hash8.restype = C.c_uint8
         L.zxo_hash8.argtypes = [C.c_void_p]
         L.zxo_hash16.restype = C.c_uint16

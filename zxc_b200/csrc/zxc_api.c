@@ -547,6 +547,30 @@ out:
     return ret;
 }
 
+/* The reference attaches the dictionary's literal table once per frame (zxc_cctx_attach_dict_huf, zxc_common.c:490):
+ * an all-zero table counts as no table, so enc_lit = 3 blocks then need one (DICT_REQUIRED); a table with a length
+ * above 11, or whose lengths are not a complete code (one symbol of length 1 excepted), fails the whole frame.
+ * Returns 1 for a usable table, 0 for none, ZXC_ERROR_CORRUPT_DATA for a bad one. */
+static int dict_huf_attach(const uint8_t* h) {
+    if (!h) return 0;
+    uint32_t kraft = 0, present = 0, any = 0, len1 = 0;
+    for (int i = 0; i < 128; i++) {
+        any |= h[i];
+        for (int k = 0; k < 2; k++) {
+            const uint32_t l = (h[i] >> (4 * k)) & 15u;
+            if (l > 11) return ZXC_ERROR_CORRUPT_DATA;
+            if (l) {
+                kraft += 1u << (11 - l);
+                present++;
+                len1 += l == 1;
+            }
+        }
+    }
+    if (!any) return 0;
+    if (kraft != (1u << 11) && !(present == 1 && len1 == 1)) return ZXC_ERROR_CORRUPT_DATA;
+    return 1;
+}
+
 static int64_t decompress_frame(zxg_ctx* g, const uint8_t* src, size_t src_size, uint8_t* dst,
                                 size_t dst_capacity, const zxc_decompress_opts_t* opts) {
     const int checksum_enabled = opts ? opts->checksum_enabled : 0;
@@ -564,6 +588,11 @@ static int64_t decompress_frame(zxg_ctx* g, const uint8_t* src, size_t src_size,
     if (w.dict_id != 0) {
         if (!dict || dict_size == 0) { ret = ZXC_ERROR_DICT_REQUIRED; goto out; }
         if (zxc_dict_id(dict, dict_size, dict_huf) != w.dict_id) { ret = ZXC_ERROR_DICT_MISMATCH; goto out; }
+    }
+    if (dict_size) {
+        const int arc = dict_huf_attach(dict_huf);
+        if (arc < 0) { ret = arc; goto out; }
+        if (arc == 0) dict_huf = NULL;
     }
     const int verify = w.has_checksum && checksum_enabled;
 
@@ -745,7 +774,7 @@ static int64_t decode_one_block(zxc_dctx* dctx, const void* src, size_t src_size
     if (!g) return ZXC_ERROR_MEMORY;
     const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
     const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
-    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
+    const uint8_t* dict_huf = NULL; /* the reference's block API attaches no literal table: enc_lit = 3 needs one */
     const int verify = opts ? opts->checksum_enabled : 0;
     if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
     uint8_t* d_in = (uint8_t*)zxg_buffer(g, ZXG_BUF_IN, src_size + 16);

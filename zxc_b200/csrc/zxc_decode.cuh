@@ -388,12 +388,12 @@ __device__ int parse_sections(const u8* pay, u32 comp, bool ghi, u32 cap, const 
         S.tok = p_data + lit_comp;
         S.offs = S.tok + tok_comp;
         if (!LEAN && enc_tok == 2) { /* level 7: Huffman-coded tokens (:1019-1022) */
-            if (n_seq + 32u > scr_tok_cap(block_cap) || tok_comp < 128) return ZXC_ERROR_CORRUPT_DATA;
-            if (n_seq) {
-                const int rc = pivco_decode(S.tok, S.tok + 128, tok_comp - 128, tok_buf, n_seq, hw, cum, cum_words, lane);
-                if (rc != ZXC_OK) return rc;
-                __syncwarp();
-            }
+            /* the reference's token buffer holds block_cap / 5 + 16 sequences (zxc_cctx_max_seq) and its PivCo decoder
+             * rejects an empty section; scr_tok_cap(block_cap) >= that + 32 */
+            if (n_seq == 0 || n_seq > block_cap / 5u + 16u || tok_comp < 128) return ZXC_ERROR_CORRUPT_DATA;
+            const int rc = pivco_decode(S.tok, S.tok + 128, tok_comp - 128, tok_buf, n_seq, hw, cum, cum_words, lane);
+            if (rc != ZXC_OK) return rc;
+            __syncwarp();
             S.tok = tok_buf;
         }
         S.ext = S.offs + (u32)sz_off;

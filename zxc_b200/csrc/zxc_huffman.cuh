@@ -20,6 +20,17 @@
  */
 #pragma once
 
+#ifndef ZXC_STAT
+#define ZXC_STAT(i, v) /* tests/simt counts events here (lane 0 only); nothing in the product build */
+#endif
+/* emulator counters of this file (tests/simt): 32 single-symbol sections, 33 lanes that took a bitmap step, 34 rank
+ * words filled, 35 verdicts, 40 + D symbols read from a flat root of depth D */
+#define HUF_FAIL()                   \
+    do {                             \
+        ZXC_STAT(35, 1);             \
+        return ZXC_ERROR_CORRUPT_DATA; \
+    } while (0)
+
 #define HUF_MAXLEN 11
 #define HUF_MAXNODES 512
 #define HUF_KIND_LEAF 0u
@@ -37,9 +48,12 @@ struct HufWork {
 };
 #define HUF_WORK_BYTES ((sizeof(HufWork) + 255u) & ~255u)
 
-__device__ __forceinline__ u32 huf_bits32(const u8* run, u32 word) { /* 32 run bits starting at bit 32*word */
-    const u8* p = run + 4u * word;
-    return (u32)p[0] | ((u32)p[1] << 8) | ((u32)p[2] << 16) | ((u32)p[3] << 24);
+/* byte k of the run area, 0 past its end: the 4-byte bitmap word and the 3-byte flat path of a symbol in the last
+ * node's run may reach past the section, which can be the end of the source buffer */
+__device__ __forceinline__ u32 huf_byte(const u8* runs, u32 rsz, u32 k) { return k < rsz ? (u32)runs[k] : 0u; }
+__device__ __forceinline__ u32 huf_bits32(const u8* runs, u32 rsz, u32 k) { /* 32 run bits starting at byte k */
+    return huf_byte(runs, rsz, k) | (huf_byte(runs, rsz, k + 1) << 8) | (huf_byte(runs, rsz, k + 2) << 16) |
+           (huf_byte(runs, rsz, k + 3) << 24);
 }
 
 /* Decodes n symbols.  lens128: 128 packed nibbles; runs/rsz: the run area; cum: cum_words rank words.
@@ -64,13 +78,13 @@ __device__ __noinline__ int pivco_decode(const u8* lens128, const u8* runs, u32 
             present++;
         }
     }
-    if (__any_sync(FULL, bad)) return ZXC_ERROR_CORRUPT_DATA;
+    if (__any_sync(FULL, bad)) HUF_FAIL();
 #pragma unroll
     for (int d = 16; d >= 1; d >>= 1) {
         kraft += __shfl_xor_sync(FULL, kraft, d);
         present += __shfl_xor_sync(FULL, present, d);
     }
-    if (present == 0) return ZXC_ERROR_CORRUPT_DATA;
+    if (present == 0) HUF_FAIL();
     u32 cnt[HUF_MAXLEN + 2];
 #pragma unroll
     for (int l = 0; l <= HUF_MAXLEN + 1; l++) cnt[l] = 0;
@@ -88,19 +102,20 @@ __device__ __noinline__ int pivco_decode(const u8* lens128, const u8* runs, u32 
         base_l += c_l;
     }
     const bool single = (present == 1 && cnt[1] == 1 && kraft == (1u << (HUF_MAXLEN - 1)));
-    if (kraft != (1u << HUF_MAXLEN) && !single) return ZXC_ERROR_CORRUPT_DATA;
+    if (kraft != (1u << HUF_MAXLEN) && !single) HUF_FAIL();
     __syncwarp();
     if (single) {
         /* one symbol of length 1: the root's bitmap must route every symbol left */
         const u32 bytes = (n + 7) >> 3;
-        if (bytes > rsz) return ZXC_ERROR_CORRUPT_DATA;
+        if (bytes > rsz) HUF_FAIL();
         u32 nz = 0;
         for (u32 k = lane; k < bytes; k += 32) {
             u32 b = runs[k];
             if (k == bytes - 1 && (n & 7u)) b &= (1u << (n & 7u)) - 1u;
             nz |= b;
         }
-        if (__any_sync(FULL, nz != 0)) return ZXC_ERROR_CORRUPT_DATA;
+        if (__any_sync(FULL, nz != 0)) HUF_FAIL();
+        ZXC_STAT(32, 1);
         const u8 sym = W->sorted[0];
         for (u32 k = lane; k < n; k += 32) out[k] = sym;
         return ZXC_OK;
@@ -125,7 +140,7 @@ __device__ __noinline__ int pivco_decode(const u8* lens128, const u8* runs, u32 
         first[HUF_MAXLEN + 1] = 0;
         lbase[HUF_MAXLEN + 1] = nodes;
         leafb[HUF_MAXLEN + 1] = leaves;
-        if (nodes > HUF_MAXNODES) return ZXC_ERROR_CORRUPT_DATA;
+        if (nodes > HUF_MAXNODES) HUF_FAIL();
     }
     if (lane <= HUF_MAXLEN + 1) {
         W->first[lane] = first[lane];
@@ -183,16 +198,17 @@ __device__ __noinline__ int pivco_decode(const u8* lens128, const u8* runs, u32 
         const u32 v = first[l] + (id - lbase[l]);
         if (kind >= 2) { /* flat root: c paths of `kind` bits */
             const u32 bytes = (c * kind + 7) >> 3;
-            if (bytes > rsz - roff) return ZXC_ERROR_CORRUPT_DATA;
+            if (bytes > rsz - roff) HUF_FAIL();
             if (lane == 0) W->runoff[id] = roff;
             roff += bytes;
             continue;
         }
         const u32 bytes = (c + 7) >> 3;
-        if (bytes > rsz - roff) return ZXC_ERROR_CORRUPT_DATA;
+        if (bytes > rsz - roff) HUF_FAIL();
         const u8* run = runs + roff;
         const u32 words = (c + 31) >> 5;
-        if (words > cum_words - coff) return ZXC_ERROR_CORRUPT_DATA;
+        if (words > cum_words - coff) HUF_FAIL();
+        ZXC_STAT(34, words);
         u32 ones = 0;
         for (u32 w0 = 0; w0 < words; w0 += 32) {
             const u32 wi = w0 + lane;
@@ -225,22 +241,25 @@ __device__ __noinline__ int pivco_decode(const u8* lens128, const u8* runs, u32 
     /* ---- every output symbol walks down from the root ---- */
     for (u32 k0 = 0; k0 < n; k0 += 32) {
         const u32 k = k0 + lane;
+        u32 flat_seen = 0, steps = 0; /* emulator counters only */
         if (k < n) {
             u32 lv = 0, v = 0, idx = k;
             for (;;) {
                 const u32 id = lbase[lv] + (v - first[lv]);
                 const u32 kind = W->kind[id];
                 if (kind == HUF_KIND_LEAF) break;
-                const u8* run = runs + W->runoff[id];
+                const u32 ro = W->runoff[id];
                 if (kind >= 2) {
-                    const u32 bp = idx * kind;
-                    u32 bits = (u32)run[bp >> 3] | ((u32)run[(bp >> 3) + 1] << 8) | ((u32)run[(bp >> 3) + 2] << 16);
+                    const u32 bp = idx * kind, b = ro + (bp >> 3);
+                    u32 bits = huf_byte(runs, rsz, b) | (huf_byte(runs, rsz, b + 1) << 8) | (huf_byte(runs, rsz, b + 2) << 16);
                     bits >>= (bp & 7u);
                     for (u32 j = 0; j < kind; j++) v = (v << 1) | ((bits >> j) & 1u);
                     lv += kind;
+                    flat_seen |= 1u << kind;
                     break;
                 }
-                const u32 word = huf_bits32(run, idx >> 5);
+                steps++;
+                const u32 word = huf_bits32(runs, rsz, ro + 4u * (idx >> 5));
                 const u32 bit = (word >> (idx & 31u)) & 1u;
                 const u32 before = cum[W->cumoff[id] + (idx >> 5)] + __popc(word & ((1u << (idx & 31u)) - 1u));
                 idx = bit ? before : idx - before;
@@ -249,6 +268,11 @@ __device__ __noinline__ int pivco_decode(const u8* lens128, const u8* runs, u32 
             }
             out[k] = W->sorted[leafb[lv] + (v - first[lv])];
         }
+        ZXC_STAT(33, __popc(__ballot_sync(FULL, steps != 0)));
+#pragma unroll
+        for (u32 D = 2; D <= HUF_MAXLEN; D++) ZXC_STAT(40 + D, __popc(__ballot_sync(FULL, (flat_seen >> D) & 1u)));
+        (void)flat_seen;
+        (void)steps;
     }
     return ZXC_OK;
 }
