@@ -144,6 +144,43 @@ template <int OFF> static inline void sts16(u32 a, u32 v) { const unsigned short
 template <int OFF> static inline void sts8(u32 a, u32 v) { smem[a + OFF] = (u8)v; }
 #endif
 
+/* L1 prefetch of the 128-byte line that holds p: a hint that never faults and returns nothing, so no instruction
+ * waits on it.  The emulator has no caches. */
+#ifdef __CUDACC__
+__device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
+#else
+static inline void prefetch_l1(const void*) {}
+#endif
+
+/* Development flavour (make NVEXTRA=-DZXC_TRACE=1 OUT=<elsewhere>): lane 0 of every warp adds clock64() deltas per
+ * phase of the sequence-centric body, and event counts, to its row of zxc_trace_acc; zxc_b200_trace_read() returns
+ * the rows (profiles/trace_decode.py).  In the product build the hooks expand to nothing. */
+#if ZXC_TRACE
+#define TRACE_SLOTS 16
+#define TRACE_ROWS 8192
+enum {
+    TR_UNPACK, TR_SCAN, TR_LIT, TR_MATCH, TR_TAIL, TR_FLUSH, TR_START, TR_END, TR_GIANT, TR_CLAIM,
+    TR_BATCHES, TR_BLOCKS, TR_M_RING, TR_M_GLOBAL, TR_M_DICT, TR_M_SEQ
+};
+__device__ unsigned long long zxc_trace_acc[TRACE_ROWS * TRACE_SLOTS];
+__device__ __forceinline__ void trace_add(u32 slot, unsigned long long v, u32 lane) {
+    const u32 row = blockIdx.x * WARPS_PER_CTA + (threadIdx.x >> 5);
+    if (lane == 0 && row < TRACE_ROWS) atomicAdd(&zxc_trace_acc[row * TRACE_SLOTS + slot], v);
+}
+#define ZXC_TRACE_DECL long long tr_t = clock64()
+#define ZXC_TRACE_MARK(slot, lane)                               \
+    do {                                                         \
+        const long long tr_n = clock64();                        \
+        trace_add(slot, (unsigned long long)(tr_n - tr_t), lane); \
+        tr_t = tr_n;                                             \
+    } while (0)
+#define ZXC_TRACE_ADD(slot, v, lane) trace_add(slot, (unsigned long long)(v), lane)
+#else
+#define ZXC_TRACE_DECL
+#define ZXC_TRACE_MARK(slot, lane)
+#define ZXC_TRACE_ADD(slot, v, lane)
+#endif
+
 #include "zxc_decode_stage.cuh"
 #define WARP_SMEM_BYTES (RING_BYTES + STAGE_BYTES) /* a warp's output ring, its staging area right behind */
 #define DECODE_SMEM_BYTES (WARPS_PER_CTA * WARP_SMEM_BYTES)
@@ -700,6 +737,8 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
     constexpr bool ghi = GHI;
     const u8* dict = HAS_DICT ? dict_in : (const u8*)0;
     const u32 dict_size = HAS_DICT ? dict_size_in : 0u;
+    ZXC_TRACE_DECL;
+    ZXC_TRACE_ADD(TR_BLOCKS, 1, lane);
     Sections S;
     const int prc = parse_sections<LEAN>(pay, comp, ghi, cap, dict_huf, scratch, scratch_cap, lane, S);
     if (prc != ZXC_OK) return prc;
@@ -788,12 +827,18 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
 #define ST_LIT_CLOSE() do { } while (0)
 #endif
 
+    ZXC_TRACE_MARK(TR_START, lane);
+
     u32 base = 0;
     while (base < n_seq) {
         /* ---- unpack tokens and offsets ---- */
         const u32 i = base + lane;
         const bool valid = i < n_seq;
         u32 ll = 0, ml = 0, off = 1;
+        /* LEAN without a dictionary: the first 512 bytes of literals from the cursor on (a batch reads 290 on the bench
+         * corpus) are requested into L1 now, so that they arrive while the tokens and offsets do and the literal pass
+         * finds them there; clamped to the literal section.  (With a dictionary both prefetches measured slower.) */
+        if (LEAN && !HAS_DICT && lane < 4u && L + 128u * lane < n_lit_avail) prefetch_l1(lit + L + 128u * lane);
 #if ZXC_STAGE
         const u32 tok_w = ghi ? 4u : 1u, off_w = enc_off ? 1u : 2u;
         const u32 tx0 = (u32)(reinterpret_cast<uintptr_t>(tok) & 15u), ox0 = (u32)(reinterpret_cast<uintptr_t>(offs) & 15u);
@@ -860,6 +905,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
         /* ---- escapes: one uniform walk over the batch's varints ---- */
         const bool e_ll = valid && ll == esc, e_ml = valid && ml == esc;
         const u32 m_ll = __ballot_sync(FULL, e_ll), m_ml = __ballot_sync(FULL, e_ml);
+        ZXC_TRACE_MARK(TR_UNPACK, lane);
         u32 k_esc = 0, epos_end = epos;
         if ((m_ll | m_ml) && use_vals) {
             u32 k = ord_base + __popc(m_ll & lt_mask) + __popc(m_ml & lt_mask);
@@ -925,6 +971,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             if (!use_vals)
                 for (u32 s = 0; s < q; s++) epos = varint_advance(ext, epos, ext_end); /* rare: re-walk */
             base += 1;
+            ZXC_TRACE_MARK(TR_GIANT, lane);
             continue;
         }
 
@@ -980,6 +1027,21 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
          * sequential order is the reference's order, so no dependency analysis is needed, and a chain of 32 dependent
          * matches costs 32 short steps instead of 32 passes. */
         const bool m_free = src_end <= (i32)O;
+        if (LEAN && !HAS_DICT && act && m_free && !near && src_lo >= 0) {
+            /* LEAN without a dictionary: the first and last source line of every free match outside the ring, requested
+             * into L1 now so that they arrive while the literal pass waits on its own loads and the match pass finds
+             * them there instead of paying a second round trip.  Both lie in output already written (below O). */
+            const u8* ps = out + src_lo;
+            const u8* pe = ps + ml - 1u;
+            prefetch_l1(ps);
+            if ((reinterpret_cast<uintptr_t>(ps) ^ reinterpret_cast<uintptr_t>(pe)) >> 7) prefetch_l1(pe);
+        }
+        ZXC_TRACE_ADD(TR_M_RING, __popc(__ballot_sync(FULL, act && near)), lane);
+        ZXC_TRACE_ADD(TR_M_GLOBAL, __popc(__ballot_sync(FULL, act && !near && src_lo >= 0)), lane);
+        ZXC_TRACE_ADD(TR_M_DICT, __popc(__ballot_sync(FULL, act && !near && src_lo < 0)), lane);
+        ZXC_TRACE_ADD(TR_M_SEQ, __popc(__ballot_sync(FULL, act && !m_free)), lane);
+        ZXC_TRACE_ADD(TR_BATCHES, 1, lane);
+        ZXC_TRACE_MARK(TR_SCAN, lane);
         /* ---- pass loop ---- */
         ZXC_STAT(0, 1);            /* batches */
         ZXC_STAT(1, m);            /* sequences */
@@ -1038,6 +1100,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
                 }
             }
             __syncwarp();
+            ZXC_TRACE_MARK(lit_pass ? TR_LIT : TR_MATCH, lane);
             if (!lit_pass) break;
             lit_pass = false;
         }
@@ -1063,12 +1126,14 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
                 __syncwarp();
             }
         }
+        ZXC_TRACE_MARK(TR_TAIL, lane);
 
         /* ---- advance and flush ---- */
         O += T;
         L += TL;
         ring_flush(w, F, O & ~511u, lane, al16);
         __syncwarp();
+        ZXC_TRACE_MARK(TR_FLUSH, lane);
 
         if (m < nvalid) {
             const u32 below = (1u << m) - 1u;
@@ -1092,6 +1157,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
     __syncwarp();
     flush_wait(lane);
     warp_copy(out + O, lit + L, rem, lane);
+    ZXC_TRACE_MARK(TR_END, lane);
     return (int)(O + rem);
 }
 
@@ -1192,9 +1258,11 @@ __global__ void __launch_bounds__(CTA_THREADS, CTAS_PER_SM) zxc_decode_kernel(co
         return;
     }
     for (;;) {
+        ZXC_TRACE_DECL;
         unsigned long long j = 0;
         if (lane == 0) j = atomicAdd(P.counter, 1ull);
         j = __shfl_sync(FULL, j, 0);
+        ZXC_TRACE_MARK(TR_CLAIM, lane);
         if (j >= P.n_jobs) break;
         const zxc_b200_job_t job = P.jobs[j];
         const int r = decode_job<UNITS, HAS_DICT, LEAN>(P, job, scratch, ring, lane);

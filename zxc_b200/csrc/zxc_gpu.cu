@@ -338,6 +338,20 @@ extern "C" int zxc_b200_device_count(void) {
 
 extern "C" uint64_t zxc_b200_launch_count(void) { return g_launches; }
 
+#if ZXC_TRACE
+/* traced build only: copies the current device's phase-trace rows (TRACE_ROWS x TRACE_SLOTS counters) to `host` and
+ * zeroes them; returns the number of counters */
+extern "C" ZXC_EXPORT int zxc_b200_trace_read(unsigned long long* host) {
+    const size_t bytes = sizeof(unsigned long long) * TRACE_ROWS * TRACE_SLOTS;
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (cudaMemcpyFromSymbol(host, zxc_trace_acc, bytes) != cudaSuccess) return -1;
+    void* d = 0;
+    if (cudaGetSymbolAddress(&d, zxc_trace_acc) != cudaSuccess || cudaMemset(d, 0, bytes) != cudaSuccess) return -1;
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    return TRACE_ROWS * TRACE_SLOTS;
+}
+#endif
+
 extern "C" int zxg_current_device(void) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) {
