@@ -88,6 +88,11 @@ ZXC_EXPORT int64_t zxc_b200_reduce_status(const int32_t* d_status, const zxc_b20
 /* Kernels launched by this library since load (for bench.py's gpu_launches). */
 ZXC_EXPORT uint64_t zxc_b200_launch_count(void);
 
+/* Phase times (ms) of the calling thread's last dictionary-training calls, for profiles/train_bench.py: upload,
+ * count, segments, host sort, pick (zxc_train_dict); slice upload, histogram encode, code lengths
+ * (zxc_train_dict_huf).  Writes min(n, 8) entries and returns their number. */
+ZXC_EXPORT int zxc_b200_train_phase_times(double* ms, int n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,9 +2,11 @@
  * zxc_dict.h -- dictionary identity, .zxd container, trainers.
  *
  * On the hot path: zxc_dict_id (binds a frame to its dictionary), load/save/
- * get_id/huf (the .zxd container).  The trainers are offline tooling outside
- * the hot-path scope (SURVEY.md section 2 row 8); they are exported for ABI
- * completeness and report ZXC_B200_ERROR_UNSUPPORTED.
+ * get_id/huf (the .zxd container).  The trainers run their data-parallel work
+ * on the GPU (k-gram count, candidate segments, greedy pick; the level-6 parses
+ * whose literals make the shared table) and return the reference's bytes and
+ * codes; without a device a valid call returns ZXC_B200_ERROR_NO_DEVICE
+ * (DESIGN.md section 7d).
  *
  * Reference interface replaced (file:line in /root/reference):
  *   zxc_dict_id          include/zxc_dict.h:52    src/lib/zxc_dict.c:35

@@ -39,7 +39,7 @@ typedef enum {
     ZXC_B200_ERROR_NO_DEVICE = -100,
     ZXC_B200_ERROR_CUDA = -101,
     /* additive: entry point exported for ABI completeness but outside the
-     * hot-path scope of this build (FILE* streaming, push streaming, trainers). */
+     * hot-path scope of this build (push streaming). */
     ZXC_B200_ERROR_UNSUPPORTED = -102
 } zxc_error_t;
 

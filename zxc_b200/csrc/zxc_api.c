@@ -186,22 +186,7 @@ const void* zxc_dict_huf(const void* buf, size_t buf_size) {
     return s + ZXC_DICT_HEADER_SIZE + csz;
 }
 
-/* offline trainers: outside the hot-path scope (SURVEY.md section 2 row 8) */
-int64_t zxc_train_dict(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
-                       void* dict_buf, size_t dict_capacity) {
-    (void)samples; (void)sample_sizes; (void)n_samples; (void)dict_buf; (void)dict_capacity;
-    return ZXC_B200_ERROR_UNSUPPORTED;
-}
-int zxc_train_dict_huf(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
-                       const void* dict, size_t dict_size, uint8_t* huf_lengths_out) {
-    (void)samples; (void)sample_sizes; (void)n_samples; (void)dict; (void)dict_size; (void)huf_lengths_out;
-    return ZXC_B200_ERROR_UNSUPPORTED;
-}
-int64_t zxc_dict_train(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
-                       void* zxd_buf, size_t zxd_capacity) {
-    (void)samples; (void)sample_sizes; (void)n_samples; (void)zxd_buf; (void)zxd_capacity;
-    return ZXC_B200_ERROR_UNSUPPORTED;
-}
+/* the trainers (zxc_train_dict, zxc_train_dict_huf, zxc_dict_train) are in zxc_train.c */
 
 /* ------------------------------------------------------------------------- */
 /* frame planning (additive public entry)                                    */

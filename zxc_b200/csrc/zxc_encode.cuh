@@ -382,26 +382,11 @@ __device__ __forceinline__ u32 seed_shared_stop(u32 dict_size, bool hash5);
 #include "zxc_encode_opt.cuh"
 static_assert(sizeof(PivcoPlan) <= ENC_PLAN_BYTES, "PivcoPlan must fit its scratch slot");
 
-/* OPT = levels 6-7 (optimal parser + entropy stage); a separate instantiation keeps the level 1-5
- * kernel at its own register budget */
-template <bool OPT>
-__device__ u32 encode_block(const EncodeParams& P, const u8* blk, u32 n, u8* dst, u8* scratch, u32* hist, u32 lane) {
-    const int level = (int)P.level;
-    const LzParams lzp = lz_params(level);
-    const bool ghi = level <= 2;
-    const u32 bs = P.block_size;
-
-    const EncLayout lay = enc_layout(bs, level);
-    u32* head = reinterpret_cast<u32*>(scratch);
-    unsigned short* chain = reinterpret_cast<unsigned short*>(scratch + ENC_HASH_SIZE * 4);
-    u8* literals = scratch + lay.literals;
-    const u32 seq_cap = lay.seq_cap;
-    u8* seqbuf = scratch + lay.seqbuf;                      /* GLO: tokens then u16 offsets; GHI: u32 words */
-    u8* extras = scratch + lay.extras;
-    u8* tokens = seqbuf;
-    unsigned short* offsets = reinterpret_cast<unsigned short*>(seqbuf + ((seq_cap + 3) & ~3u));
-    u32* seqwords = reinterpret_cast<u32*>(seqbuf);
-
+/* The warp's match tables for one block, and the bytes the parse reads: with a dictionary, the seeded tables cloned
+ * and [dict | block] materialised in scratch (the block at position dict_size); without, cleared tables and the
+ * block itself. */
+__device__ __forceinline__ const u8* enc_block_tables(const EncodeParams& P, const EncLayout& lay, int level, const u8* blk,
+                                                      u32 n, u8* scratch, u32* head, unsigned short* chain, u32 lane) {
     const u32 base = P.dict ? P.dict_size : 0u; /* the dictionary is logically prepended to the block */
     const u8* src = blk; /* block start is 4-byte aligned (block_size multiple of 4096, aligned base) */
     if (base) {
@@ -426,6 +411,31 @@ __device__ u32 encode_block(const EncodeParams& P, const u8* blk, u32 n, u8* dst
         for (u32 k = lane; k < ENC_HASH_SIZE / 4; k += 32) reinterpret_cast<uint4*>(head)[k] = make_uint4(0, 0, 0, 0);
     }
     __syncwarp();
+    return src;
+}
+
+/* OPT = levels 6-7 (optimal parser + entropy stage); a separate instantiation keeps the level 1-5
+ * kernel at its own register budget */
+template <bool OPT>
+__device__ u32 encode_block(const EncodeParams& P, const u8* blk, u32 n, u8* dst, u8* scratch, u32* hist, u32 lane) {
+    const int level = (int)P.level;
+    const LzParams lzp = lz_params(level);
+    const bool ghi = level <= 2;
+    const u32 bs = P.block_size;
+
+    const EncLayout lay = enc_layout(bs, level);
+    u32* head = reinterpret_cast<u32*>(scratch);
+    unsigned short* chain = reinterpret_cast<unsigned short*>(scratch + ENC_HASH_SIZE * 4);
+    u8* literals = scratch + lay.literals;
+    const u32 seq_cap = lay.seq_cap;
+    u8* seqbuf = scratch + lay.seqbuf;                      /* GLO: tokens then u16 offsets; GHI: u32 words */
+    u8* extras = scratch + lay.extras;
+    u8* tokens = seqbuf;
+    unsigned short* offsets = reinterpret_cast<unsigned short*>(seqbuf + ((seq_cap + 3) & ~3u));
+    u32* seqwords = reinterpret_cast<u32*>(seqbuf);
+
+    const u32 base = P.dict ? P.dict_size : 0u; /* the dictionary is logically prepended to the block */
+    const u8* src = enc_block_tables(P, lay, level, blk, n, scratch, head, chain, lane);
 
     const u32 iend = base + n;
     u32 ip = base, anchor = base;

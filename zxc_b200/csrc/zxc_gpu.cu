@@ -12,6 +12,7 @@
  *                       and out; only with ZXC_B200_DECODE_V2=1 (it measured 6.7x slower on the H100, DESIGN.md section 3c); what
  *                       it defers (entropy-coded sections, checksum verification) goes to zxc_decode_kernel
  * Encode: zxc_encode.cuh (levels 1-5), zxc_encode_opt.cuh (levels 6-7).
+ * Dictionary training: zxc_train.cuh (zxg_train_* at the end of this file).
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -26,6 +27,7 @@
 #include "zxc_decode.cuh"
 #include "zxc_decode2.cuh"
 #include "zxc_encode.cuh"
+#include "zxc_train.cuh"
 
 /* ========================================================================= */
 /* host side: device bring-up, contexts, copies, launches                    */
@@ -1300,5 +1302,302 @@ extern "C" int zxg_encode_body(zxg_ctx* c, const uint8_t* h_src, uint64_t src_si
         if (rc == ZXC_OK) rc = zxg_sync(c);
     }
     free(h_offs);
+    return rc;
+}
+
+/* ------------------------------------------------------------------------- */
+/* dictionary training (zxc_train.c drives these; kernels in zxc_train.cuh)   */
+/* ------------------------------------------------------------------------- */
+static_assert(sizeof(TrainSeg) == sizeof(zxg_seg_t), "TrainSeg and zxg_seg_t are the same record");
+
+static __thread double t_train_ms[ZXG_T_N];
+extern "C" double* zxg_train_times(void) { return t_train_ms; }
+
+/* Packs n host pieces back to back into d_dst through the context's pinned bounce buffers: one DMA per 32 MiB, not
+ * one per piece (a million 100-byte samples is an ordinary training input).  A NULL piece of non-zero size reads as
+ * zeros. */
+static int h2d_gather(zxg_ctx* c, u8* d_dst, const void* const* pieces, const size_t* sizes, size_t n) {
+    const int rc = ensure_pins(c);
+    if (rc != ZXC_OK) return rc;
+    size_t fill = 0, d_off = 0;
+    int slot = 0;
+    cudaEventSynchronize(c->pin_ev[slot]);
+    for (size_t i = 0; i < n; i++) {
+        const u8* s = (const u8*)pieces[i];
+        size_t left = sizes[i];
+        while (left) {
+            const size_t take = left < PIN_CHUNK - fill ? left : PIN_CHUNK - fill;
+            if (s) {
+                pool_memcpy(c->device, (u8*)c->pin[slot] + fill, s, take);
+                s += take;
+            } else {
+                memset((u8*)c->pin[slot] + fill, 0, take);
+            }
+            fill += take;
+            left -= take;
+            if (fill == PIN_CHUNK) {
+                if (cudaMemcpyAsync(d_dst + d_off, c->pin[slot], fill, cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
+                    return ZXC_B200_ERROR_CUDA;
+                cudaEventRecord(c->pin_ev[slot], c->stream);
+                d_off += fill;
+                fill = 0;
+                slot ^= 1;
+                cudaEventSynchronize(c->pin_ev[slot]); /* the previous use of this bounce buffer */
+            }
+        }
+    }
+    if (fill) {
+        if (cudaMemcpyAsync(d_dst + d_off, c->pin[slot], fill, cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
+            return ZXC_B200_ERROR_CUDA;
+        cudaEventRecord(c->pin_ev[slot], c->stream);
+    }
+    return ZXC_OK;
+}
+
+struct train_events {
+    cudaEvent_t ev[8];
+    int n;
+};
+static int tev_init(train_events* T, int n) {
+    T->n = 0;
+    for (int i = 0; i < n; i++) {
+        if (cudaEventCreate(&T->ev[i]) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+        T->n++;
+    }
+    return ZXC_OK;
+}
+static double tev_ms(train_events* T, int a, int b) {
+    float ms = 0;
+    cudaEventElapsedTime(&ms, T->ev[a], T->ev[b]);
+    return ms;
+}
+static void tev_free(train_events* T) {
+    for (int i = 0; i < T->n; i++) cudaEventDestroy(T->ev[i]);
+}
+
+static int grid_cap(unsigned long long want, u32 per_sm) {
+    const unsigned long long cap = (unsigned long long)(g_sm_count > 0 ? g_sm_count : 132) * per_sm;
+    return (int)(want < 1 ? 1 : (want < cap ? want : cap));
+}
+
+/* device layout of the content trainer, behind the corpus: ZXG_BUF_AUX = [freq u32 x 65536 | result words | starts |
+ * kept segments]; ZXG_BUF_JOBS = [ordered segments | hash offsets | chunk starts | picks | output] */
+#define TRN_RES_OFF ((size_t)TRN_HASH_SIZE * 4)
+#define TRN_STARTS_OFF (TRN_RES_OFF + 256)
+static size_t trn_kept_off(u32 n_starts) { return (TRN_STARTS_OFF + (size_t)n_starts * sizeof(TrainSeg) + 255) & ~(size_t)255; }
+
+extern "C" int zxg_train_segments(zxg_ctx* c, const void* const* samples, const size_t* sizes, size_t n_samples,
+                                  uint64_t corpus_size, uint64_t freq_stride, uint64_t seg_stride, uint32_t n_starts,
+                                  uint32_t seg_alloc, zxg_seg_t* h_segs, uint32_t* n_segs) {
+    *n_segs = 0;
+    u8* d_corpus = (u8*)zxg_buffer(c, ZXG_BUF_IN, (size_t)corpus_size + 16);
+    u8* aux = (u8*)zxg_buffer(c, ZXG_BUF_AUX, trn_kept_off(n_starts) + (size_t)seg_alloc * sizeof(TrainSeg) + 256);
+    if (!d_corpus || !aux) return ZXC_ERROR_MEMORY;
+    u32* d_freq = (u32*)aux;
+    u32* d_res = (u32*)(aux + TRN_RES_OFF);
+    TrainSeg* d_starts = (TrainSeg*)(aux + TRN_STARTS_OFF);
+    TrainSeg* d_kept = (TrainSeg*)(aux + trn_kept_off(n_starts));
+    train_events T;
+    int rc = tev_init(&T, 4);
+    if (rc == ZXC_OK) {
+        cudaEventRecord(T.ev[0], c->stream);
+        rc = h2d_gather(c, d_corpus, samples, sizes, n_samples);
+    }
+    if (rc == ZXC_OK && (cudaMemsetAsync(d_corpus + corpus_size, 0, 16, c->stream) != cudaSuccess ||
+                         cudaMemsetAsync(d_freq, 0, TRN_RES_OFF + 256, c->stream) != cudaSuccess))
+        rc = ZXC_B200_ERROR_CUDA;
+    if (rc == ZXC_OK) {
+        cudaEventRecord(T.ev[1], c->stream);
+        const unsigned long long kgram_limit = corpus_size - TRN_K + 1;
+        const unsigned long long n_count = (kgram_limit + freq_stride - 1) / freq_stride;
+        zxc_train_count_kernel<<<grid_cap((n_count + 255) / 256, 16), 256, 0, c->stream>>>(d_corpus, kgram_limit, freq_stride,
+                                                                                          d_freq);
+        cudaEventRecord(T.ev[2], c->stream);
+        if (cudaFuncSetAttribute(zxc_train_seg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TRN_SEG_SMEM) != cudaSuccess)
+            rc = ZXC_B200_ERROR_CUDA;
+    }
+    if (rc == ZXC_OK) {
+        zxc_train_seg_kernel<<<grid_cap(((unsigned long long)n_starts + 31) / 32, 1), TRN_CTA, TRN_SEG_SMEM, c->stream>>>(
+            d_corpus, corpus_size, seg_stride, n_starts, d_freq, d_starts);
+        zxc_train_compact_kernel<<<1, TRN_CTA, 0, c->stream>>>(d_starts, n_starts, seg_alloc, d_kept, d_res);
+        __atomic_add_fetch(&g_launches, 3, __ATOMIC_RELAXED);
+        cudaEventRecord(T.ev[3], c->stream);
+        u32 n = 0;
+        if (cudaMemcpyAsync(&n, d_res, 4, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
+            cudaStreamSynchronize(c->stream) != cudaSuccess)
+            rc = ZXC_B200_ERROR_CUDA;
+        else if (n && (cudaMemcpyAsync(h_segs, d_kept, (size_t)n * sizeof(TrainSeg), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
+                       cudaStreamSynchronize(c->stream) != cudaSuccess))
+            rc = ZXC_B200_ERROR_CUDA;
+        *n_segs = n;
+    }
+    if (rc == ZXC_OK) {
+        t_train_ms[ZXG_T_UPLOAD] = tev_ms(&T, 0, 1);
+        t_train_ms[ZXG_T_COUNT] = tev_ms(&T, 1, 2);
+        t_train_ms[ZXG_T_SEGMENTS] = tev_ms(&T, 2, 3);
+    } else {
+        fprintf(stderr, "libzxc (CUDA build): dictionary training failed: %s\n", cudaGetErrorString(cudaGetLastError()));
+    }
+    tev_free(&T);
+    return rc;
+}
+
+extern "C" int zxg_train_pick(zxg_ctx* c, uint64_t corpus_size, const zxg_seg_t* h_sorted, uint32_t n_segs, uint32_t capacity,
+                              uint8_t* h_out, uint32_t* filled) {
+    *filled = 0;
+    if (n_segs == 0) return ZXC_OK;
+    /* hash offsets in pick order, and the chunks of at most TRN_CHUNK hashes the pick stages at a time */
+    u32* h_idx = (u32*)malloc(((size_t)n_segs + 1) * 2 * sizeof(u32));
+    if (!h_idx) return ZXC_ERROR_MEMORY;
+    u32* hoff = h_idx;
+    u32* chunk_first = h_idx + n_segs + 1;
+    u32 n_chunks = 0, acc = 0;
+    for (u32 j = 0; j < n_segs; j++) {
+        const u32 nk = h_sorted[j].len / TRN_K;
+        if (j == 0 || acc - hoff[chunk_first[n_chunks - 1]] + nk > TRN_CHUNK) chunk_first[n_chunks++] = j;
+        hoff[j] = acc;
+        acc += nk;
+    }
+    hoff[n_segs] = acc;
+    chunk_first[n_chunks] = n_segs;
+    const size_t o_hoff = ((size_t)n_segs * sizeof(TrainSeg) + 255) & ~(size_t)255;
+    const size_t o_chunk = (o_hoff + ((size_t)n_segs + 1) * 4 + 255) & ~(size_t)255;
+    const size_t o_picks = (o_chunk + ((size_t)n_chunks + 1) * 4 + 255) & ~(size_t)255;
+    const size_t o_out = (o_picks + (size_t)n_segs * sizeof(TrainPick) + 255) & ~(size_t)255;
+    u8* jb = (u8*)zxg_buffer(c, ZXG_BUF_JOBS, o_out + 65536 + 16);
+    unsigned short* d_hash = (unsigned short*)zxg_buffer(c, ZXG_BUF_SCRATCH, (size_t)acc * 2 + 16);
+    const u8* d_corpus = (const u8*)zxg_buffer(c, ZXG_BUF_IN, (size_t)corpus_size + 16);
+    u8* aux = (u8*)c->buf[ZXG_BUF_AUX];
+    if (!jb || !d_hash || !d_corpus || !aux) {
+        free(h_idx);
+        return ZXC_ERROR_MEMORY;
+    }
+    TrainSeg* d_seg = (TrainSeg*)jb;
+    u32* d_hoff = (u32*)(jb + o_hoff);
+    u32* d_chunk = (u32*)(jb + o_chunk);
+    TrainPick* d_picks = (TrainPick*)(jb + o_picks);
+    u8* d_out = jb + o_out;
+    u32* d_res = (u32*)(aux + TRN_RES_OFF) + 4;
+    train_events T;
+    int rc = tev_init(&T, 2);
+    if (rc == ZXC_OK &&
+        (cudaMemcpyAsync(d_seg, h_sorted, (size_t)n_segs * sizeof(TrainSeg), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+         cudaMemcpyAsync(d_hoff, hoff, ((size_t)n_segs + 1) * 4, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+         cudaMemcpyAsync(d_chunk, chunk_first, ((size_t)n_chunks + 1) * 4, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+         cudaFuncSetAttribute(zxc_train_pick_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TRN_PICK_SMEM) != cudaSuccess))
+        rc = ZXC_B200_ERROR_CUDA;
+    u32 res[2] = {0, 0};
+    if (rc == ZXC_OK) {
+        cudaEventRecord(T.ev[0], c->stream);
+        zxc_train_hash_kernel<<<grid_cap(((unsigned long long)n_segs + 7) / 8, 8), 256, 0, c->stream>>>(d_corpus, d_seg, d_hoff,
+                                                                                                     n_segs, d_hash);
+        zxc_train_pick_kernel<<<1, TRN_CTA, TRN_PICK_SMEM, c->stream>>>(d_seg, d_hoff, d_hash, d_chunk, n_chunks, (const u32*)aux,
+                                                                        capacity, d_picks, d_res);
+        __atomic_add_fetch(&g_launches, 2, __ATOMIC_RELAXED);
+        cudaEventRecord(T.ev[1], c->stream);
+        if (cudaMemcpyAsync(res, d_res, 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
+            cudaStreamSynchronize(c->stream) != cudaSuccess)
+            rc = ZXC_B200_ERROR_CUDA;
+    }
+    if (rc == ZXC_OK && res[0]) {
+        zxc_train_emit_kernel<<<grid_cap(((unsigned long long)res[0] + 7) / 8, 8), 256, 0, c->stream>>>(d_corpus, d_picks, res[0],
+                                                                                                      res[1], d_out);
+        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+        if (cudaMemcpyAsync(h_out, d_out, res[1], cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
+            cudaStreamSynchronize(c->stream) != cudaSuccess)
+            rc = ZXC_B200_ERROR_CUDA;
+    }
+    if (rc == ZXC_OK) {
+        t_train_ms[ZXG_T_PICK] = tev_ms(&T, 0, 1);
+        *filled = res[1];
+    } else {
+        fprintf(stderr, "libzxc (CUDA build): dictionary training failed: %s\n", cudaGetErrorString(cudaGetLastError()));
+    }
+    tev_free(&T);
+    free(h_idx);
+    return rc;
+}
+
+extern "C" int zxg_train_tail(zxg_ctx* c, uint64_t corpus_size, uint32_t bytes, uint8_t* h_out) {
+    const u8* d_corpus = (const u8*)zxg_buffer(c, ZXG_BUF_IN, (size_t)corpus_size + 16);
+    if (!d_corpus) return ZXC_ERROR_MEMORY;
+    if (cudaMemcpyAsync(h_out, d_corpus + corpus_size - bytes, bytes, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
+        cudaStreamSynchronize(c->stream) != cudaSuccess)
+        return ZXC_B200_ERROR_CUDA;
+    return ZXC_OK;
+}
+
+extern "C" int zxg_train_literals(zxg_ctx* c, const void* const* pieces, const size_t* sizes, size_t n, const void* h_dict,
+                                  uint32_t dict_size, uint32_t* h_freq) {
+    memset(h_freq, 0, 256 * sizeof(uint32_t));
+    if (n == 0) return ZXC_OK;
+    const u32 bs = 4096u, level = 6u; /* the reference trains at ZXC_LEVEL_DENSITY on 4 KiB slices */
+    uint64_t total = 0;
+    TrainSlice* h_sl = (TrainSlice*)malloc(n * sizeof(TrainSlice));
+    if (!h_sl) return ZXC_ERROR_MEMORY;
+    for (size_t i = 0; i < n; i++) {
+        h_sl[i].off = total;
+        h_sl[i].len = (u32)sizes[i];
+        h_sl[i].pad = 0;
+        total += sizes[i];
+    }
+    const size_t wstride = enc_layout(bs, (int)level).total;
+    const int grid = grid_cap((n + ENC_WARPS_PER_CTA - 1) / ENC_WARPS_PER_CTA, ENC_CTAS_PER_SM);
+    u8* d_src = (u8*)zxg_buffer(c, ZXG_BUF_IN, (size_t)total + 64);
+    TrainSlice* d_sl = (TrainSlice*)zxg_buffer(c, ZXG_BUF_JOBS, n * sizeof(TrainSlice));
+    u8* d_scratch = (u8*)zxg_buffer(c, ZXG_BUF_SCRATCH, (size_t)grid * ENC_WARPS_PER_CTA * wstride);
+    u32* d_freq = (u32*)zxg_buffer(c, ZXG_BUF_AUX, 256 * sizeof(u32));
+    const size_t dpad = ((size_t)dict_size + 16 + 255) & ~(size_t)255;
+    const size_t dtot = dpad + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2 + 256;
+    u8* d_dict = (u8*)zxg_buffer(c, ZXG_BUF_DICT, dtot);
+    if (!d_src || !d_sl || !d_scratch || !d_freq || !d_dict) {
+        free(h_sl);
+        return ZXC_ERROR_MEMORY;
+    }
+    train_events T;
+    int rc = tev_init(&T, 3);
+    if (rc == ZXC_OK) {
+        cudaEventRecord(T.ev[0], c->stream);
+        rc = h2d_gather(c, d_src, pieces, sizes, n);
+    }
+    if (rc == ZXC_OK &&
+        (cudaMemsetAsync(d_src + total, 0, 64, c->stream) != cudaSuccess ||
+         cudaMemcpyAsync(d_sl, h_sl, n * sizeof(TrainSlice), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+         cudaMemsetAsync(d_freq, 0, 256 * sizeof(u32), c->stream) != cudaSuccess ||
+         cudaMemsetAsync(d_dict, 0, dtot, c->stream) != cudaSuccess ||
+         cudaMemsetAsync(c->counter, 0, sizeof(unsigned long long), c->stream) != cudaSuccess))
+        rc = ZXC_B200_ERROR_CUDA;
+    if (rc == ZXC_OK) rc = zxg_h2d(c, d_dict, h_dict, dict_size);
+    if (rc == ZXC_OK) {
+        cudaEventRecord(T.ev[1], c->stream);
+        EncodeParams P;
+        memset(&P, 0, sizeof P);
+        P.src = d_src;
+        P.scratch = d_scratch;
+        P.counter = c->counter;
+        P.dict = d_dict;
+        P.seed_head = (const u32*)(d_dict + dpad);
+        P.seed_chain = (const unsigned short*)(d_dict + dpad + (size_t)ENC_HASH_SIZE * 4);
+        P.scratch_stride = wstride;
+        P.block_size = bs;
+        P.n_blocks = (u32)n;
+        P.level = level;
+        P.dict_size = dict_size;
+        zxc_seed_kernel<<<1, 32, 0, c->stream>>>(d_dict, dict_size, level, (u32*)P.seed_head, (unsigned short*)P.seed_chain);
+        zxc_train_lit_kernel<<<grid, ENC_CTA_THREADS, 0, c->stream>>>(P, d_sl, d_freq);
+        __atomic_add_fetch(&g_launches, 2, __ATOMIC_RELAXED);
+        cudaEventRecord(T.ev[2], c->stream);
+        if (cudaMemcpyAsync(h_freq, d_freq, 256 * sizeof(u32), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
+            cudaStreamSynchronize(c->stream) != cudaSuccess)
+            rc = ZXC_B200_ERROR_CUDA;
+    }
+    if (rc == ZXC_OK) {
+        t_train_ms[ZXG_T_SLICES] = tev_ms(&T, 0, 1);
+        t_train_ms[ZXG_T_HIST] = tev_ms(&T, 1, 2);
+    } else {
+        fprintf(stderr, "libzxc (CUDA build): dictionary table training failed: %s\n", cudaGetErrorString(cudaGetLastError()));
+    }
+    tev_free(&T);
+    free(h_sl);
     return rc;
 }
