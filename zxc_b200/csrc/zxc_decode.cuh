@@ -68,6 +68,12 @@ typedef int32_t i32;
 #ifndef CTAS_PER_SM
 #define CTAS_PER_SM 7u            /* register-limited (72 regs x 128 threads); 112 KB of rings, rest is L1 */
 #endif
+#ifndef LEAN_CTAS_PER_SM
+#define LEAN_CTAS_PER_SM CTAS_PER_SM /* the lean instance's own launch bounds (DESIGN.md section 9) */
+#endif
+#ifndef LEAN_SMEM_PAD
+#define LEAN_SMEM_PAD 0u /* development: extra dynamic shared memory per lean CTA, to move the carve-out step alone */
+#endif
 
 #define BT_RAW 0
 #define BT_GLO 1
@@ -782,9 +788,15 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
      * live in the rank-table area of the scratch, idle once the sections are parsed; a section too long for it
      * keeps the per-batch walk. */
     u32* vals = reinterpret_cast<u32*>(scratch + scr_lit_cap(scratch_cap) + scr_tok_cap(scratch_cap) + (u32)HUF_WORK_BYTES);
-    const bool use_vals = ext_end != 0u && 4ull * ext_end <= scr_cum_cap(scratch_cap);
+    /* LEAN: an extras section too long for the table goes to the general instance (nothing is written yet), so the
+     * batch loop below carries neither the varint cursor nor its walk; without extras every escape reads 0 from the
+     * empty table, as the reference reads 0 past the section's end */
+    if constexpr (LEAN) {
+        if (4ull * ext_end > scr_cum_cap(scratch_cap)) return D2_DEFER_STATUS;
+    }
+    const bool use_vals = LEAN || (ext_end != 0u && 4ull * ext_end <= scr_cum_cap(scratch_cap));
     u32 n_val = 0, ord_base = 0;
-    if (use_vals) {
+    if (use_vals && (!LEAN || ext_end != 0u)) {
         const u32 seg = max(4u, (ext_end + 31u) / 32u);
         const u32 nseg = (ext_end + seg - 1u) / seg;
         const u32 lo = lane * seg, hi = min(ext_end, lo + seg);
@@ -878,7 +890,13 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             if (!ghi) {
                 a = tok[i];
 #if ZXC_ALIGNED_LD
-                if (enc_off) b = (u32)offs[i];
+                if (LEAN) {
+                    /* raw tokens: the offsets follow them, so the loop holds no pointer of their own */
+                    const u32 oi = n_seq + (enc_off ? i : 2u * i);
+                    if (enc_off) b = (u32)tok[oi];
+                    else if ((reinterpret_cast<uintptr_t>(tok) + n_seq) & 1u) b = ld16(tok + oi);
+                    else b = (u32)*reinterpret_cast<const unsigned short*>(tok + oi);
+                } else if (enc_off) b = (u32)offs[i];
                 else if (reinterpret_cast<uintptr_t>(offs) & 1u) b = ld16(offs + 2 * (size_t)i);
                 else b = (u32)reinterpret_cast<const unsigned short*>(offs)[i];
 #else
@@ -1206,10 +1224,10 @@ __device__ int decode_job(const DecodeParams& P, const zxc_b200_job_t& job, u8* 
 }
 
 /* LEAN: decode_job<LEAN>; each job it defers is marked D2_DEFER_STATUS and listed for a DEFERRED launch that follows.
- * The lean instance runs at the general one's 7 CTAs per SM: at 8 (64 registers) and 10 (48) it spilled more and
- * measured slower (DESIGN.md section 9). */
+ * The lean instance has its own CTAs per SM (LEAN_CTAS_PER_SM), 7 like the general one: at 8 (64 registers) it still
+ * spills, and spills cost more than the eighth CTA gains (DESIGN.md section 9). */
 template <bool UNITS, bool DEFERRED, bool HAS_DICT, bool LEAN>
-__global__ void __launch_bounds__(CTA_THREADS, CTAS_PER_SM) zxc_decode_kernel(const DecodeParams P) {
+__global__ void __launch_bounds__(CTA_THREADS, LEAN ? LEAN_CTAS_PER_SM : CTAS_PER_SM) zxc_decode_kernel(const DecodeParams P) {
     extern __shared__ __align__(16) u8 smem[];
     const u32 lane = threadIdx.x & 31;
     const u32 wic = threadIdx.x >> 5;

@@ -570,14 +570,18 @@ extern "C" int zxg_d2h(zxg_ctx* c, void* h_dst, const void* d_src, size_t bytes)
     return ZXC_OK;
 }
 
-/* resident decode CTAs per SM: CTAS_PER_SM unless ZXC_B200_DECODE_CTAS (1..CTAS_PER_SM) says fewer --
+/* the larger of the lean and the general instance's CTAs per SM: the decode grid and the per-warp scratch are sized
+ * for it (the lean launch comes first and decodes nearly every block) */
+#define DECODE_CTAS_MAX (LEAN_CTAS_PER_SM > CTAS_PER_SM ? LEAN_CTAS_PER_SM : CTAS_PER_SM)
+
+/* resident decode CTAs per SM: DECODE_CTAS_MAX unless ZXC_B200_DECODE_CTAS (1..DECODE_CTAS_MAX) says fewer --
  * a tuning knob: fewer warps keep fewer 64 KiB output windows alive in L2 (DESIGN.md section 9) */
 static u32 decode_ctas_per_sm(void) {
     static int cached = 0;
     if (cached == 0) {
         const char* e = getenv("ZXC_B200_DECODE_CTAS");
         const int v = e ? atoi(e) : 0;
-        cached = (v >= 1 && v <= (int)CTAS_PER_SM) ? v : (int)CTAS_PER_SM;
+        cached = (v >= 1 && v <= (int)DECODE_CTAS_MAX) ? v : (int)DECODE_CTAS_MAX;
     }
     return (u32)cached;
 }
@@ -639,7 +643,7 @@ static size_t d2_spill_bytes(const D2Config* c) {
 
 extern "C" size_t zxc_b200_decode_scratch_size(uint32_t block_size) {
     if (zxg_init() != ZXC_OK) return 0;
-    const size_t warps = (size_t)g_sm_count * CTAS_PER_SM * WARPS_PER_CTA;
+    const size_t warps = (size_t)g_sm_count * DECODE_CTAS_MAX * WARPS_PER_CTA;
     size_t n = warps * scratch_stride_for(block_size) + 512; /* room to align the regions behind it to 256 bytes */
     D2Config c;
     if (d2_config(block_size, &c)) n += d2_spill_bytes(&c) + 256;
@@ -771,8 +775,20 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
     if (!verify && !units && !(P.flags & FLAG_DEFERRED)) {
         /* launch 1: the lean instance decodes the RAW blocks and the GLO blocks without Huffman sections and lists the
          * rest; launch 2 below: the general instance decodes the listed jobs (its warps exit at once when there are none) */
-        if (has_dict) zxc_decode_kernel<false, false, true, true><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
-        else zxc_decode_kernel<false, false, false, true><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
+#ifdef LEAN_CARVEOUT
+        /* development: the shared-memory share of the unified L1 / shared array, in percent, as a hint to the driver */
+        static int carveout_done = 0;
+        if (!carveout_done) {
+            cudaFuncSetAttribute(zxc_decode_kernel<false, false, true, true>,
+                                 cudaFuncAttributePreferredSharedMemoryCarveout, LEAN_CARVEOUT);
+            cudaFuncSetAttribute(zxc_decode_kernel<false, false, false, true>,
+                                 cudaFuncAttributePreferredSharedMemoryCarveout, LEAN_CARVEOUT);
+            carveout_done = 1;
+        }
+#endif
+        const u32 lean_smem = DECODE_SMEM_BYTES + LEAN_SMEM_PAD;
+        if (has_dict) zxc_decode_kernel<false, false, true, true><<<grid, CTA_THREADS, lean_smem, st>>>(P);
+        else zxc_decode_kernel<false, false, false, true><<<grid, CTA_THREADS, lean_smem, st>>>(P);
         __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
         if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
         P.flags |= FLAG_DEFERRED;
