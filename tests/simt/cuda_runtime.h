@@ -3,9 +3,10 @@
  *
  * A stand-in for <cuda_runtime.h> that lets the product's DEVICE code (the .cuh files under zxc_b200/csrc) compile with
  * g++ and run on the CPU, one emulated warp = 32 fibers in one OS thread (simt_rt.h).  Every warp-level
- * primitive (__shfl*_sync, __ballot_sync, __syncwarp, ...) is a rendezvous of the 32 fibers: a lane that
- * reaches one parks, the scheduler resumes the other lanes in a (seeded) random order until all have
- * arrived, computes every lane's result and lets them continue.  Between two rendezvous the lanes run one
+ * primitive (__shfl*_sync, __ballot_sync, __syncwarp, ...) is a rendezvous of the lanes its mask names: a lane
+ * that reaches one parks, the scheduler resumes the other lanes in a (seeded) random order until every lane of
+ * the mask has arrived at the same primitive with the same mask, computes the group's results over the mask
+ * and lets it continue; disjoint groups (partial masks) complete independently.  Between two rendezvous the lanes run one
  * after another in that random order, so code that needs an ordering the source does not ask for with a
  * __syncwarp() shows up as a mismatch -- and a lane that skips a rendezvous the others take deadlocks
  * loudly.  Nothing here is linked into libzxc.so; the tests use it to check the kernels' logic against
@@ -37,31 +38,32 @@ struct dim3 { unsigned x, y, z; };
 #define threadIdx (simt::cur().tid)
 #define blockIdx (simt::cur().bid)
 #define blockDim (simt::cur().bdim)
+static const dim3 gridDim = {1, 1, 1}; /* the harnesses launch the warps of one grid-stride loop as a grid of one block */
 
-/* ---- warp primitives: full-mask only, which is all the product code uses ---- */
-static inline void __syncwarp(unsigned mask = 0xFFFFFFFFu) { (void)mask; simt::rendezvous(simt::OP_SYNC, 0, 0); }
-static inline unsigned __ballot_sync(unsigned, int pred) { return (unsigned)simt::rendezvous(simt::OP_BALLOT, pred != 0, 0); }
-static inline int __any_sync(unsigned, int pred) { return simt::rendezvous(simt::OP_BALLOT, pred != 0, 0) != 0; }
-static inline int __all_sync(unsigned, int pred) { return (unsigned)simt::rendezvous(simt::OP_BALLOT, pred != 0, 0) == simt::live_mask(); }
-static inline unsigned __reduce_max_sync(unsigned, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_MAX, v, 0); }
-static inline unsigned __reduce_min_sync(unsigned, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_MIN, v, 0); }
-static inline unsigned __reduce_add_sync(unsigned, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_ADD, v, 0); }
-static inline unsigned __reduce_or_sync(unsigned, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_OR, v, 0); }
-static inline unsigned __match_any_sync(unsigned, unsigned long long v) { return (unsigned)simt::rendezvous(simt::OP_MATCH, v, 0); }
+/* ---- warp primitives: the mask names the lanes that take part (simt_rt.cc run_warp) ---- */
+static inline void __syncwarp(unsigned mask = 0xFFFFFFFFu) { simt::rendezvous(simt::OP_SYNC, 0, 0, mask); }
+static inline unsigned __ballot_sync(unsigned m, int pred) { return (unsigned)simt::rendezvous(simt::OP_BALLOT, pred != 0, 0, m); }
+static inline int __any_sync(unsigned m, int pred) { return simt::rendezvous(simt::OP_BALLOT, pred != 0, 0, m) != 0; }
+static inline int __all_sync(unsigned m, int pred) { return (unsigned)simt::rendezvous(simt::OP_BALLOT, pred != 0, 0, m) == m; }
+static inline unsigned __reduce_max_sync(unsigned m, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_MAX, v, 0, m); }
+static inline unsigned __reduce_min_sync(unsigned m, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_MIN, v, 0, m); }
+static inline unsigned __reduce_add_sync(unsigned m, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_ADD, v, 0, m); }
+static inline unsigned __reduce_or_sync(unsigned m, unsigned v) { return (unsigned)simt::rendezvous(simt::OP_OR, v, 0, m); }
+static inline unsigned __match_any_sync(unsigned m, unsigned long long v) { return (unsigned)simt::rendezvous(simt::OP_MATCH, v, 0, m); }
 
-template <class T> static inline T simt_shfl(int op, T v, unsigned arg) {
+template <class T> static inline T simt_shfl(int op, unsigned mask, T v, unsigned arg) {
     static_assert(sizeof(T) <= 8, "shuffle of at most 64 bits");
     uint64_t raw = 0;
     memcpy(&raw, &v, sizeof(T));
-    raw = simt::rendezvous(op, raw, arg);
+    raw = simt::rendezvous(op, raw, arg, mask);
     T r;
     memcpy(&r, &raw, sizeof(T));
     return r;
 }
-template <class T> static inline T __shfl_sync(unsigned, T v, int src, int width = 32) { (void)width; return simt_shfl(simt::OP_SHFL_IDX, v, (unsigned)src & 31u); }
-template <class T> static inline T __shfl_up_sync(unsigned, T v, unsigned d, int width = 32) { (void)width; return simt_shfl(simt::OP_SHFL_UP, v, d); }
-template <class T> static inline T __shfl_down_sync(unsigned, T v, unsigned d, int width = 32) { (void)width; return simt_shfl(simt::OP_SHFL_DOWN, v, d); }
-template <class T> static inline T __shfl_xor_sync(unsigned, T v, int m, int width = 32) { (void)width; return simt_shfl(simt::OP_SHFL_XOR, v, (unsigned)m); }
+template <class T> static inline T __shfl_sync(unsigned m, T v, int src, int width = 32) { (void)width; return simt_shfl(simt::OP_SHFL_IDX, m, v, (unsigned)src & 31u); }
+template <class T> static inline T __shfl_up_sync(unsigned m, T v, unsigned d, int width = 32) { (void)width; return simt_shfl(simt::OP_SHFL_UP, m, v, d); }
+template <class T> static inline T __shfl_down_sync(unsigned m, T v, unsigned d, int width = 32) { (void)width; return simt_shfl(simt::OP_SHFL_DOWN, m, v, d); }
+template <class T> static inline T __shfl_xor_sync(unsigned m, T v, int x, int width = 32) { (void)width; return simt_shfl(simt::OP_SHFL_XOR, m, v, (unsigned)x); }
 
 /* ---- scalar intrinsics ---- */
 static inline int __popc(unsigned v) { return __builtin_popcount(v); }

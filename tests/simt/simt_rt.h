@@ -17,6 +17,7 @@ struct LaneCtx {
     int op;            /* pending rendezvous */
     uint64_t val;
     unsigned arg;
+    unsigned mask;     /* the lanes that take part in it */
     uint64_t result;
     bool done;
 };
@@ -33,11 +34,12 @@ struct Warp {
 extern thread_local Warp* g_warp;
 
 static inline LaneCtx& cur() { return g_warp->lane[g_warp->current]; }
-unsigned live_mask();
-uint64_t rendezvous(int op, uint64_t val, unsigned arg);
+uint64_t rendezvous(int op, uint64_t val, unsigned arg, unsigned mask);
 
 /* runs body(lane) on 32 fibers to completion; block/threads describe threadIdx for lane l as first_tid + l.
- * seed != 0: lanes are resumed in a random order between rendezvous; seed == 0: lane order. */
+ * seed != 0: lanes are resumed in a random order between rendezvous; seed == 0: lane order.  Returns the number of
+ * rendezvous groups completed.  Aborts (a finding: undefined behaviour on the GPU) when a lane names a mask without
+ * itself, a mask names a lane that has exited, or the parked lanes can complete no group. */
 uint64_t run_warp(const std::function<void(unsigned)>& body, unsigned first_tid, unsigned block_idx, unsigned block_dim,
                   uint64_t seed);
 

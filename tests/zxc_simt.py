@@ -90,3 +90,78 @@ def lean_emu(tmp_path_factory):
                                           C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint64,
                                           C.c_void_p]
     return lib
+
+
+def build_encoder(out_dir):
+    """tests/simt/simt_encode.cc -- the encode kernels' source on the fiber warp emulator -- compiled into out_dir"""
+    so = os.path.join(str(out_dir), "libzxc_simt_encode.so")
+    root = os.path.dirname(HERE)
+    extra = os.environ.get("ZXC_SIMT_EXTRA", "").split()  # e.g. -I<dir> ahead of zxc_b200/csrc for a variant encoder
+    r = subprocess.run(["g++", *extra, "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall", "-Wno-unknown-pragmas",
+                        "-Wno-unused-function", "-I.", "-I" + os.path.join(root, "include"),
+                        "-I" + os.path.join(root, "zxc_b200", "csrc"), "-o", so, "simt_encode.cc", "simt_rt.cc"],
+                       cwd=SIMT_DIR, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+    assert r.returncode == 0 and "warning" not in r.stdout, r.stdout[-3000:]
+    lib = C.CDLL(so)
+    lib.simt_encode.restype = C.c_uint64
+    lib.simt_encode.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_int, C.c_void_p, C.c_uint32, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+    lib.simt_enc_staging_stride.restype = C.c_uint32
+    lib.simt_enc_staging_stride.argtypes = [C.c_uint32]
+    lib.simt_enc_guard_pages.argtypes = [C.c_int]
+    return lib
+
+
+@pytest.fixture(scope="session")
+def enc_emu(tmp_path_factory):
+    return build_encoder(tmp_path_factory.mktemp("simt_encode"))
+
+
+def encode_stats(lib):
+    """the encode harness's ZXC_STAT / ZXC_LANE_STAT counters (zxc_encode.cuh, zxc_encode_opt.cuh: 64 and up)"""
+    return (C.c_uint64 * 128).in_dll(lib, "simt_stat")
+
+
+class Encoded:
+    def __init__(self, blocks, body, rendezvous, stray_slot, stray_scratch):
+        self.blocks, self.body, self.rendezvous = blocks, body, rendezvous
+        self.stray_slot, self.stray_scratch = stray_slot, stray_scratch
+
+
+def encode_frame(lib, data, level, block_size, checksum=0, dict=None, dict_huf=None, seed=1):
+    """the frame body zxg_encode_body would emit for `data` (one emulated warp per block): an Encoded with the per-block
+    bytes, the compacted body, the rendezvous count and the stores found outside the slots / outside the scratch.
+    dict_huf is the dictionary's packed 128-byte literal table, unpacked here as zxc_compress does."""
+    src = np.ascontiguousarray(np.frombuffer(bytes(data), np.uint8) if not isinstance(data, np.ndarray) else data)
+    nb = (src.size + block_size - 1) // block_size
+    stride = lib.simt_enc_staging_stride(block_size)
+    slots = np.zeros(max(nb * stride, 1), np.uint8)
+    sizes = (C.c_uint32 * max(nb, 1))()
+    body = np.zeros(max(nb * stride, 1), np.uint8)
+    stray = (C.c_uint64 * 2)()
+    d = np.frombuffer(bytes(dict), np.uint8) if dict else None
+    lens = None
+    if dict_huf is not None and any(dict_huf):
+        h = np.frombuffer(bytes(dict_huf), np.uint8)
+        lens = np.empty(256, np.uint8)
+        lens[0::2], lens[1::2] = h & 15, h >> 4
+    rv = lib.simt_encode(src.ctypes.data if src.size else None, src.size, block_size, level, checksum,
+                         d.ctypes.data if d is not None else None, d.size if d is not None else 0,
+                         lens.ctypes.data if lens is not None else None, slots.ctypes.data, sizes, body.ctypes.data, seed,
+                         stray)
+    blocks = [slots[j * stride:j * stride + sizes[j]].tobytes() for j in range(nb)]
+    total = sum(sizes[j] for j in range(nb))
+    return Encoded(blocks, body[:total].tobytes(), rv, stray[0], stray[1])
+
+
+def frame_blocks(frame, checksum):
+    """the data blocks of a frame (16-byte file header, then blocks of an 8-byte header -- type in byte 0, payload size
+    in bytes 3..6 -- the payload and, with checksums, 4 more bytes) up to the EOF block"""
+    fb = bytes(frame)
+    cks = checksum
+    out, p = [], 16
+    while p + 8 <= len(fb) and fb[p] != 255:
+        n = 8 + int.from_bytes(fb[p + 3:p + 7], "little") + (4 if cks else 0)
+        out.append(fb[p:p + n])
+        p += n
+    return out

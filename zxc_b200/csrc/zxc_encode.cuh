@@ -32,6 +32,10 @@
 #include "zxc_decode.cuh" /* u8/u32, FULL, warp_checksum, ld helpers */
 #include "zxc_hufenc.h"
 
+#ifndef ZXC_LANE_STAT
+#define ZXC_LANE_STAT(i, v) /* tests/simt counts one lane's own event here (every lane); nothing in the product build */
+#endif
+
 #define ENC_HUFWORK_BYTES ((sizeof(zxh_work_t) + 255u) & ~(size_t)255u)
 #define ENC_PLAN_BYTES 8192u
 
@@ -200,11 +204,13 @@ __device__ Match find_best_match(const u8* src, u32 ip, u32 iend, u32 search_lim
     int attempts = p.search_depth;
     if (match_idx != 0) {
         if (skip_head) {
+            ZXC_STAT(92, 1); /* a head whose tag differs is skipped */
             const u32 delta = chain[match_idx & (ENC_WINDOW - 1)];
             match_idx = delta ? match_idx - delta : 0;
             attempts--;
         }
         while (match_idx > 0) {
+            ZXC_STAT(78, attempts >= 0 && ip - match_idx > ENC_MAX_DIST); /* candidates beyond the window */
             if (attempts-- < 0 || ip - match_idx > ENC_MAX_DIST) break;
             const u32 delta = chain[match_idx & (ENC_WINDOW - 1)];
             const u32 next_idx = match_idx - delta;
@@ -253,6 +259,7 @@ __device__ Match find_best_match(const u8* src, u32 ip, u32 iend, u32 search_lim
             int att = p.lazy_attempts;
             bool first = true;
             while (idx > 0) {
+                ZXC_STAT(78, att > 0 && lp - idx > ENC_MAX_DIST);
                 if (att-- <= 0 || lp - idx > ENC_MAX_DIST) break;
                 if ((!first || !skip_first) && ldu32(src, idx) == v) {
                     /* only compared against best.len + 1/2 < 130: one 128-byte step is enough */
@@ -265,7 +272,10 @@ __device__ Match find_best_match(const u8* src, u32 ip, u32 iend, u32 search_lim
                 first = false;
             }
         }
-        if (max_lazy[0] > best.len + 1 || max_lazy[1] > best.len + 2) best.found = false;
+        if (max_lazy[0] > best.len + 1 || max_lazy[1] > best.len + 2) {
+            ZXC_STAT(79, 1); /* lazy replacements */
+            best.found = false;
+        }
     }
     return best;
 }
@@ -403,6 +413,7 @@ __device__ __forceinline__ const u8* enc_block_tables(const EncodeParams& P, con
         src = comb;
         __syncwarp();
         if (base >= 5 && lane == 0) { /* positions whose hash window reaches into the block */
+            ZXC_STAT(91, 1);
             const bool h5 = level >= 3;
             for (u32 i = seed_shared_stop(base, h5); i < base - 4; i++) seed_step(src, i, (base - 4) / 2, h5, head, chain);
         }
@@ -462,6 +473,7 @@ __device__ u32 encode_block(const EncodeParams& P, const u8* blk, u32 n, u8* dst
             if (ip + step >= search_limit) step = 1;
             const Match m = find_best_match(src, ip, iend, search_limit, anchor, head, chain, level, lzp, lane);
             if (m.found) {
+                ZXC_STAT(81, m.backtrack != 0); /* backtracked starts */
                 ip -= m.backtrack;
                 const u32 ll = ip - anchor;
                 const u32 ml = m.len - 5;
@@ -492,6 +504,7 @@ __device__ u32 encode_block(const EncodeParams& P, const u8* blk, u32 n, u8* dst
                 if (!ghi && m.len > 2 && level > 4) { /* level 5: also index match_end - 2 (:1231-1248) */
                     const u32 match_end = ip + m.len;
                     if (match_end + 7 < iend) {
+                        ZXC_STAT(82, 1);
                         const u32 pos_u = match_end - 2;
                         const u32 h_u = enc_hash(ldu64(src, pos_u), true);
                         const u32 prev = head[h_u];
@@ -506,6 +519,7 @@ __device__ u32 encode_block(const EncodeParams& P, const u8* blk, u32 n, u8* dst
                 ip += m.len;
                 anchor = ip;
             } else {
+                ZXC_STAT(80, step > 1); /* step skips */
                 ip += step;
             }
         }
@@ -548,6 +562,7 @@ __device__ u32 encode_block(const EncodeParams& P, const u8* blk, u32 n, u8* dst
             __syncwarp();
             have_hist = true;
             if (build_section_lengths(freq_lit, cl_lit, cap, hw, lane)) {
+                ZXC_STAT(93, 1); /* literal Huffman codes built */
                 const u32 pay = pivco_plan(freq_lit, cl_lit, plan, lane);
                 if (pay != 0xFFFFFFFFu) {
                     const u32 j = pay + 128u + ((lit_c * 4u) >> 8); /* zxc_ss_prem_huf_q8 */
@@ -597,9 +612,15 @@ __device__ u32 encode_block(const EncodeParams& P, const u8* blk, u32 n, u8* dst
         const u32 pad = behind < 32 ? 32 - behind : 0;
         w = 8 + 12 + (ghi ? lit_c : desc + sz_lit) + behind + pad;
     }
+    ZXC_STAT(83, w >= n); /* RAW blocks */
     if (w >= n) {
         /* expansion: store RAW (:2055-2058) */
     } else if (!ghi) {
+        ZXC_STAT(84, enc_lit == ENC_RLE);
+        ZXC_STAT(85, enc_lit == ENC_HUF);
+        ZXC_STAT(86, enc_lit == ENC_HUF_DICT);
+        ZXC_STAT(87, enc_tok == ENC_HUF);
+        ZXC_STAT(88, off8);
         if (lane == 0) {
             st32(p, seq_c);
             st32(p + 4, lit_c);

@@ -259,6 +259,7 @@ __device__ u32 pivco_write(const u8* sym, u32 n, const u8* code_len, PivcoPlan* 
                 const int leader = __ffs(grp) - 1;
                 u32 base = 0;
                 if ((int)lane == leader) {
+                    ZXC_LANE_STAT(90, __popc(grp) > 1); /* lanes on one node take consecutive slots */
                     base = T->wpos[id];
                     T->wpos[id] = base + __popc(grp);
                 }
@@ -270,6 +271,7 @@ __device__ u32 pivco_write(const u8* sym, u32 n, const u8* code_len, PivcoPlan* 
                     d++;
                     if (d >= l) active = false;
                 } else { /* flat root of depth `kind`: the remaining path, first branch in bit 0 */
+                    ZXC_LANE_STAT(89, 1);
                     const u32 low = v & ((1u << kind) - 1u);
                     const u32 r = __brev(low) >> (32u - kind);
                     if (r) or_bits(out + T->runoff[id], slot * kind, r);
@@ -379,6 +381,7 @@ __device__ __forceinline__ void dp_front_step(DpFront& F, u64* dp, u32 n, u32 pi
         }
     }
     if (span_end >= 64) { /* beyond the register front */
+        ZXC_STAT(75, 1);
         for (u32 L = 64 - i + lane; L <= L_max; L += 32) {
             const u32 nxt = cur + opt_match_cost(L);
             if (nxt < (u32)(dp[pi + L] >> 32)) dp[pi + L] = ((u64)nxt << 32) | (L << 16) | offb;
@@ -475,7 +478,10 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
                 oldc[my] = chain[slot];
                 const u32 dist = pos - midx[k];
                 chain[slot] = (midx[k] != 0 && dist < ENC_WINDOW) ? (unsigned short)dist : 0;
-                if (lane == 31u - (u32)__clz(grp[k])) head[hh[k]] = pos; /* provisional: undone on truncation */
+                if (lane == 31u - (u32)__clz(grp[k])) { /* provisional: undone on truncation */
+                    ZXC_LANE_STAT(70, __popc(grp[k]) > 1); /* insert groups of more than one lane */
+                    head[hh[k]] = pos;
+                }
             }
             __syncwarp();
         }
@@ -488,6 +494,7 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
     {                                                                                        \
         const u32 jj = ((q) - pos0) & (ENC_WINDOW - 1);                                      \
         const u32 cv_ = chain[(q) & (ENC_WINDOW - 1)];                                       \
+        ZXC_LANE_STAT(68, jj > (my) && jj < nact);                                           \
         out = (jj > (my) && jj < nact) ? (u32)oldc[jj] : cv_;                                \
     }
 #pragma unroll
@@ -499,6 +506,7 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
             att[k] = lzp.search_depth;
             idx[k] = midx[k]; /* 0 for inactive lanes */
             if (skip_head[k]) {
+                ZXC_LANE_STAT(92, 1);
                 u32 delta;
                 OPT_RDCHAIN(idx[k], 32u * k + lane, delta);
                 idx[k] = delta ? idx[k] - delta : 0;
@@ -513,6 +521,7 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
 #pragma unroll
             for (int k = 0; k < OPT_K; k++) {
                 const u32 pos = pos0 + 32u * k + lane;
+                ZXC_LANE_STAT(77, idx[k] > 0 && att[k] >= 0 && pos - idx[k] > ENC_MAX_DIST);
                 if (idx[k] > 0 && (att[k]-- < 0 || pos - idx[k] > ENC_MAX_DIST)) idx[k] = 0;
                 const u32 q = idx[k]; /* q == 0 reads slot 0 / byte c_len: harmless, ignored below */
                 const u32 jj = (q - pos0) & (ENC_WINDOW - 1);
@@ -524,7 +533,10 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
             for (int k = 0; k < OPT_K; k++) {
                 const u32 q = idx[k];
                 const u32 jj = (q - pos0) & (ENC_WINDOW - 1);
-                if (jj > 32u * k + lane && jj < nact) delta[k] = oc[k];
+                if (jj > 32u * k + lane && jj < nact) {
+                    ZXC_LANE_STAT(69, q != 0); /* a link the batch has already overwritten */
+                    delta[k] = oc[k];
+                }
             }
 #pragma unroll
             for (int k = 0; k < OPT_K; k++) {
@@ -596,6 +608,7 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
                     u32 rl = 0;
                     bool eq;
                     if (posi - rk_pos < rk_len) {
+                        ZXC_STAT(71, 1);
                         rl = rk_len - (posi - rk_pos);
                         eq = rl >= 4;
 #ifdef ZXC_OPT_PROFILE
@@ -603,6 +616,8 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
 #endif
                     } else {
                         const u32 sp = __shfl_sync(FULL, spec[k], i);
+                        ZXC_STAT(72, sp == last_off);
+                        ZXC_STAT(73, sp != last_off);
 #ifdef ZXC_OPT_PROFILE
                         if (sp == last_off) n_spec++; else n_load++;
 #endif
@@ -616,6 +631,7 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
                     if (eq) {
                         const bool fin = rl >= (u32)lzp.sufficient_len || posi + rl >= iend;
                         if (fin || !found || len <= rl) { /* ties go to the repeat offset */
+                            ZXC_STAT(74, found && len == rl);
                             found = true;
                             len = rl;
                             ref = posi - last_off;
@@ -629,7 +645,10 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
                     rk_pos = posi; /* len is the full common prefix at this offset */
                     rk_len = len;
                     L_max = len > n - pi ? n - pi : len;
-                    if (L_max > 65535u) L_max = 65535u;
+                    if (L_max > 65535u) {
+                        ZXC_STAT(76, 1);
+                        L_max = 65535u;
+                    }
                     offb = (off - 1u) & 0xFFFFu;
                 }
 #ifdef ZXC_OPT_PROFILE
@@ -650,6 +669,8 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
         }
         __syncwarp();
         OPT_T(4)
+        ZXC_STAT(64, 1);
+        ZXC_STAT(65, valid != nact);
         if (valid != nact) {
             /* undo the inserts past `valid`, highest first: each hash ends up pointing at what its lowest
              * undone position had found there */
@@ -660,7 +681,11 @@ __device__ OptOut optimal_parse(const u8* src, u32 base, u32 n, u32* head, unsig
                 const u32 invm = __ballot_sync(FULL, inv);
                 if (inv) {
                     chain[(pos0 + my) & (ENC_WINDOW - 1)] = oldc[my];
-                    if ((grp[k] & invm & ((1u << lane) - 1u)) == 0) head[hh[k]] = midx[k];
+                    ZXC_LANE_STAT(67, 1);
+                    if ((grp[k] & invm & ((1u << lane) - 1u)) == 0) {
+                        ZXC_LANE_STAT(66, 1); /* the lowest undone position of its hash restores the head */
+                        head[hh[k]] = midx[k];
+                    }
                 }
                 __syncwarp();
             }
