@@ -7,6 +7,7 @@
  * walks the frame once into a job table (one entry per block), the kernel
  * decodes all jobs in one launch.  They are what bench.py times for the
  * HBM-resident `value`, and what a multi-GPU caller shards by block range.
+ * zxc_b200_compress_device is the encode counterpart: HBM in, a complete frame (and its job table) in HBM out.
  *
  * Nothing here exists in the reference; adding symbols passes its ABI policy
  * (abidiff --no-added-syms, .github/workflows/abi-check.yml:128).
@@ -84,6 +85,34 @@ ZXC_EXPORT int zxc_b200_decode_blocks(const void* d_src, void* d_dst, const zxc_
  * `stream`. */
 ZXC_EXPORT int64_t zxc_b200_reduce_status(const int32_t* d_status, const zxc_b200_job_t* d_jobs,
                                           uint32_t n_jobs, void* stream);
+
+/* Device scratch that zxc_b200_compress_device needs to compress src_size bytes at these options with the
+ * full resident encode grid (0: invalid options, or no device).  At level 6-7 with 64 KiB blocks that is about
+ * 1.3 MiB per warp on top of roughly 2 x src_size; a smaller scratch also works, see below. */
+ZXC_EXPORT size_t zxc_b200_encode_scratch_size(uint64_t src_size, const zxc_compress_opts_t* opts);
+
+/* Compress src_size bytes at d_src into a complete ZXC frame at d_dst, on `stream`, asynchronously.
+ *   opts       as for zxc_compress: level, block_size, checksum_enabled, seekable, and dict / dict_size /
+ *              dict_huf in HOST memory (the dictionary is read before the call returns)
+ *   d_scratch  device scratch; with less than zxc_b200_encode_scratch_size(...) bytes the encode runs as many
+ *              warps as the scratch holds (same output, slower); below one warp's worth the call fails
+ *   d_result   one device int64: the frame size, or ZXC_ERROR_DST_TOO_SMALL when the frame does not fit
+ *              dst_capacity (the contents of d_dst are then unspecified)
+ *   d_jobs     NULL, or ceil(src_size / block_size) entries in device memory: the decode plan of the emitted
+ *              frame (what zxc_b200_plan_frame returns for it), ready for zxc_b200_decode_blocks
+ * d_dst[0 .. *d_result) equals what zxc_compress returns for the same bytes and options.  d_src and d_dst may have
+ * any alignment; nothing outside [d_src, d_src + src_size) is read, and nothing outside d_dst[0 .. dst_capacity),
+ * the scratch, *d_result and d_jobs is written.  There is no host synchronisation, no copy through the host and
+ * no allocation in the call; without a dictionary it may be captured in a CUDA graph.  Kernel launches per call
+ * (zxc_b200_launch_count): 6 when src_size > 0 (encode, three assembly kernels, compaction, finish), plus one
+ * dictionary-seeding kernel with a dictionary; 1 for an empty input.
+ * Returns ZXC_OK once enqueued, or what the host decides, in zxc_compress's order: ZXC_ERROR_NULL_INPUT (also for a
+ * NULL d_scratch or d_result), ZXC_ERROR_DICT_TOO_LARGE, ZXC_ERROR_BAD_BLOCK_SIZE (also for too many blocks),
+ * ZXC_B200_ERROR_NO_DEVICE, ZXC_ERROR_DST_TOO_SMALL (dst_capacity below header + trailer), ZXC_ERROR_CORRUPT_DATA
+ * (malformed dict_huf), then ZXC_ERROR_MEMORY when the scratch holds less than one warp. */
+ZXC_EXPORT int zxc_b200_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                                        const zxc_compress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                                        int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
 
 /* Kernels launched by this library since load (for bench.py's gpu_launches). */
 ZXC_EXPORT uint64_t zxc_b200_launch_count(void);

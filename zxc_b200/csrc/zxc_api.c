@@ -796,18 +796,9 @@ int64_t zxc_decompress_block_safe(zxc_dctx* dctx, const void* src, const size_t 
 /* encode entry points: frame assembly on the host around zxg_encode_body     */
 /* (all levels encode on the GPU; without a device they fail loudly).        */
 /* ------------------------------------------------------------------------- */
-static int64_t compress_frame(zxg_ctx* g, const uint8_t* src, size_t src_size, uint8_t* dst, size_t dst_capacity,
-                              int level, size_t block_size, int checksum, int seekable, const uint8_t* dict,
-                              size_t dict_size, const uint8_t* dict_huf) {
-    const uint64_t nb64 = (src_size + block_size - 1) / block_size;
-    if (nb64 > 0xFFFFFFFFull - 2) return ZXC_ERROR_BAD_BLOCK_SIZE;
-    const uint32_t nb = (uint32_t)nb64;
-    const size_t trailer = ZXF_BLOCK_HDR + ((seekable && nb > 0) ? zxc_seek_table_size(nb) : 0) + ZXC_FILE_FOOTER_SIZE;
-    if (dst_capacity < ZXC_FILE_HEADER_SIZE + trailer) return ZXC_ERROR_DST_TOO_SMALL;
-    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
-    /* the dictionary's shared literal table (zxc_cctx_attach_dict_huf, zxc_common.c:490-513): an
-     * all-zero table means "none"; a malformed one fails the call */
-    uint8_t huf_lens[256];
+/* the dictionary's shared literal table (zxc_cctx_attach_dict_huf, zxc_common.c:490-513): an all-zero table means
+ * "none" (*have = 0); a malformed one fails the call.  Fills huf_lens with one length per byte. */
+static int unpack_dict_huf(const uint8_t* dict_huf, uint8_t huf_lens[256], int* have) {
     int have_huf = 0;
     if (dict_huf) {
         for (int i = 0; i < ZXC_HUF_TABLE_SIZE; i++) {
@@ -821,7 +812,35 @@ static int64_t compress_frame(zxg_ctx* g, const uint8_t* src, size_t src_size, u
             have_huf = 1;
         }
     }
-    int r = zxf_write_file_header(dst, dst_capacity, block_size, checksum, did);
+    *have = have_huf;
+    return ZXC_OK;
+}
+
+/* the SEK block's header: its payload is one ZXF_SEEK_ENTRY per block */
+static void seek_table_header(uint8_t* dst, uint32_t num_blocks) {
+    zxf_write_block_header(dst, ZXF_BLOCK_HDR, ZXF_BT_SEK, num_blocks * ZXF_SEEK_ENTRY);
+}
+
+/* bytes of a frame around its body: file header, EOF block, SEK table, footer */
+static uint64_t frame_fixed_bytes(uint32_t nb, int seekable) {
+    return ZXC_FILE_HEADER_SIZE + ZXF_BLOCK_HDR + ((seekable && nb > 0) ? zxc_seek_table_size(nb) : 0) +
+           ZXC_FILE_FOOTER_SIZE;
+}
+
+static int64_t compress_frame(zxg_ctx* g, const uint8_t* src, size_t src_size, uint8_t* dst, size_t dst_capacity,
+                              int level, size_t block_size, int checksum, int seekable, const uint8_t* dict,
+                              size_t dict_size, const uint8_t* dict_huf) {
+    const uint64_t nb64 = (src_size + block_size - 1) / block_size;
+    if (nb64 > 0xFFFFFFFFull - 2) return ZXC_ERROR_BAD_BLOCK_SIZE;
+    const uint32_t nb = (uint32_t)nb64;
+    const size_t trailer = frame_fixed_bytes(nb, seekable) - ZXC_FILE_HEADER_SIZE;
+    if (dst_capacity < ZXC_FILE_HEADER_SIZE + trailer) return ZXC_ERROR_DST_TOO_SMALL;
+    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
+    uint8_t huf_lens[256];
+    int have_huf = 0;
+    int r = unpack_dict_huf(dict_huf, huf_lens, &have_huf);
+    if (r != ZXC_OK) return r;
+    r = zxf_write_file_header(dst, dst_capacity, block_size, checksum, did);
     if (r < 0) return r;
     uint32_t* sizes = nb ? (uint32_t*)malloc((size_t)nb * sizeof *sizes) : NULL;
     if (nb && !sizes) return ZXC_ERROR_MEMORY;
@@ -871,6 +890,66 @@ int64_t zxc_compress(const void* src, const size_t src_size, void* dst, const si
                                      checksum, seekable, dict, dict_size, dict_huf);
     zxg_release(g);
     return r;
+}
+
+/* ---- device to device (include/zxc_b200.h) ---- */
+/* zxc_compress's option checks, in its order; fills the effective level, block size and block count */
+static int device_opts(uint64_t src_size, const zxc_compress_opts_t* opts, int* level, size_t* block_size,
+                       uint32_t* n_blocks) {
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    *level = level_clamp(opts ? opts->level : 0);
+    *block_size = (opts && opts->block_size) ? opts->block_size : ZXC_BLOCK_SIZE_DEFAULT;
+    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    if (!zxf_valid_block_size(*block_size)) return ZXC_ERROR_BAD_BLOCK_SIZE;
+    const uint64_t nb64 = (src_size + *block_size - 1) / *block_size;
+    if (nb64 > 0xFFFFFFFFull - 2) return ZXC_ERROR_BAD_BLOCK_SIZE;
+    *n_blocks = (uint32_t)nb64;
+    return ZXC_OK;
+}
+
+size_t zxc_b200_encode_scratch_size(uint64_t src_size, const zxc_compress_opts_t* opts) {
+    int level;
+    size_t bs;
+    uint32_t nb;
+    if (device_opts(src_size, opts, &level, &bs, &nb) != ZXC_OK) return 0;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    return zxg_encode_scratch_bytes(src_size, (uint32_t)bs, level, nb, (uint32_t)dict_size);
+}
+
+int zxc_b200_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                             const zxc_compress_opts_t* opts, void* d_scratch, size_t scratch_size, int64_t* d_result,
+                             zxc_b200_job_t* d_jobs, void* stream) {
+    if (!d_dst || dst_capacity == 0 || (src_size > 0 && !d_src) || !d_scratch || !d_result) return ZXC_ERROR_NULL_INPUT;
+    int level;
+    size_t block_size;
+    uint32_t nb;
+    int rc = device_opts(src_size, opts, &level, &block_size, &nb);
+    if (rc != ZXC_OK) return rc;
+    rc = zxg_init();
+    if (rc != ZXC_OK) return rc;
+    const int checksum = opts ? opts->checksum_enabled : 0;
+    const int seekable = opts ? opts->seekable : 0;
+    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
+    zxg_frame_bytes_t fb;
+    memset(&fb, 0, sizeof fb);
+    fb.fixed = frame_fixed_bytes(nb, seekable);
+    fb.dst_capacity = dst_capacity;
+    fb.seekable = seekable && nb > 0;
+    if (dst_capacity < fb.fixed) return ZXC_ERROR_DST_TOO_SMALL;
+    uint8_t huf_lens[256];
+    int have_huf = 0;
+    rc = unpack_dict_huf(dict_huf, huf_lens, &have_huf);
+    if (rc != ZXC_OK) return rc;
+    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
+    zxf_write_file_header(fb.header, sizeof fb.header, block_size, checksum, did);
+    zxf_write_block_header(fb.eof, sizeof fb.eof, ZXF_BT_EOF, 0);
+    if (fb.seekable) seek_table_header(fb.sek, nb);
+    zxf_write_footer(fb.footer, sizeof fb.footer, src_size, 0, checksum);
+    return zxg_compress_device(d_src, src_size, d_dst, (uint32_t)block_size, level, checksum, nb, dict,
+                               (uint32_t)dict_size, have_huf ? huf_lens : NULL, &fb, d_scratch, scratch_size, d_result,
+                               d_jobs, stream);
 }
 
 int64_t zxc_compress_cctx(zxc_cctx* cctx, const void* src, size_t src_size, void* dst, size_t dst_capacity,
@@ -1132,7 +1211,7 @@ int64_t zxc_write_seek_table(uint8_t* dst, const size_t dst_capacity, const uint
     const size_t total = zxc_seek_table_size(num_blocks);
     if (dst_capacity < total) return ZXC_ERROR_DST_TOO_SMALL;
     if (!dst || !comp_sizes) return ZXC_ERROR_NULL_INPUT;
-    zxf_write_block_header(dst, dst_capacity, ZXF_BT_SEK, num_blocks * ZXF_SEEK_ENTRY);
+    seek_table_header(dst, num_blocks);
     for (uint32_t i = 0; i < num_blocks; i++) zxf_st32(dst + ZXF_BLOCK_HDR + 4 * (size_t)i, comp_sizes[i]);
     return (int64_t)total;
 }

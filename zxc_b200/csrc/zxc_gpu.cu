@@ -11,7 +11,8 @@
  *   zxc_decode2_kernel  (zxc_decode2.cuh) one CTA per block of <= 64 KiB, window in shared memory, cp.async.bulk in
  *                       and out; only with ZXC_B200_DECODE_V2=1 (it measured 6.7x slower on the H100, DESIGN.md section 3c); what
  *                       it defers (entropy-coded sections, checksum verification) goes to zxc_decode_kernel
- * Encode: zxc_encode.cuh (levels 1-5), zxc_encode_opt.cuh (levels 6-7).
+ * Encode: zxc_encode.cuh (levels 1-5), zxc_encode_opt.cuh (levels 6-7); the frame of a device-to-device compress
+ * is assembled by zxc_assemble.cuh.
  * Dictionary training: zxc_train.cuh (zxg_train_* at the end of this file).
  */
 #include <cuda_runtime.h>
@@ -27,6 +28,7 @@
 #include "zxc_decode.cuh"
 #include "zxc_decode2.cuh"
 #include "zxc_encode.cuh"
+#include "zxc_assemble.cuh"
 #include "zxc_train.cuh"
 
 /* ========================================================================= */
@@ -1223,6 +1225,95 @@ extern "C" int zxg_decode_staged(zxg_ctx* c, const uint8_t* h_src, zxg_fetch_fn 
 /* ------------------------------------------------------------------------- */
 static u32 enc_staging_stride(u32 bs) { return ((bs + 8u + 68u + 4u) + 255u) & ~255u; }
 
+/* dictionary region of an encode: [dict (padded)] [seeded head 128 KB] [seeded chain 128 KB] [256 literal lengths] */
+static size_t enc_dict_pad(u32 dict_size) { return ((size_t)dict_size + 16 + 255) & ~(size_t)255; }
+static size_t enc_dict_bytes(u32 dict_size) {
+    return enc_dict_pad(dict_size) + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2 + 256;
+}
+
+/* warps of the full resident encode grid for n_blocks blocks (a multiple of ENC_WARPS_PER_CTA) */
+static u32 enc_full_warps(u32 n_blocks) {
+    const u32 ctas_needed = (n_blocks + ENC_WARPS_PER_CTA - 1) / ENC_WARPS_PER_CTA;
+    const u32 resident = (u32)(g_sm_count > 0 ? g_sm_count : 132) * ENC_CTAS_PER_SM;
+    return (ctas_needed < resident ? ctas_needed : resident) * ENC_WARPS_PER_CTA;
+}
+
+/* One block encode on stream `st` with the given device buffers: d_src is 16-byte aligned with 64 zero bytes behind
+ * src_size, d_scratch holds `warps` per-warp slots of enc_layout(block_size, level).total bytes, d_dict (when
+ * dict_size) holds enc_dict_bytes(dict_size).  The host dictionary (<= ZXC_DICT_SIZE_MAX bytes) and literal lengths
+ * are copied in here.  Launches the seed kernel (dictionary only) and the encode kernel: `warps` warps, in CTAs of
+ * ENC_WARPS_PER_CTA when there are that many, else one CTA of `warps` warps (the kernel indexes its scratch by
+ * global warp and claims blocks through *counter, so any warp count gives the same output). */
+struct EncLaunch {
+    const u8* d_src;
+    uint64_t src_size;
+    u32 block_size, n_blocks;
+    int level, checksum;
+    u8* d_stage;
+    u32* d_sizes;
+    u8* d_scratch;
+    u32 warps;
+    unsigned long long* counter;
+    u8* d_dict;
+    const void* h_dict;
+    u32 dict_size;
+    const uint8_t* h_dict_huf_lens;
+};
+static int launch_encode(const EncLaunch& E, cudaStream_t st) {
+    EncodeParams P;
+    P.src = E.d_src;
+    P.staging = E.d_stage;
+    P.out_size = E.d_sizes;
+    P.scratch = E.d_scratch;
+    P.counter = E.counter;
+    P.dict = NULL;
+    P.seed_head = NULL;
+    P.seed_chain = NULL;
+    P.dict_huf_lens = NULL;
+    if (E.h_dict && E.dict_size) {
+        u8* d_dict = E.d_dict;
+        const size_t dpad = enc_dict_pad(E.dict_size);
+        if (cudaMemsetAsync(d_dict, 0, enc_dict_bytes(E.dict_size), st) != cudaSuccess ||
+            cudaMemcpyAsync(d_dict, E.h_dict, E.dict_size, cudaMemcpyHostToDevice, st) != cudaSuccess)
+            return ZXC_B200_ERROR_CUDA;
+        P.dict = d_dict;
+        P.seed_head = (const u32*)(d_dict + dpad);
+        P.seed_chain = (const unsigned short*)(d_dict + dpad + (size_t)ENC_HASH_SIZE * 4);
+        if (E.h_dict_huf_lens && E.level >= 6) { /* the shared literal table, one length per byte */
+            u8* d_lens = d_dict + dpad + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2;
+            if (cudaMemcpyAsync(d_lens, E.h_dict_huf_lens, 256, cudaMemcpyHostToDevice, st) != cudaSuccess)
+                return ZXC_B200_ERROR_CUDA;
+            P.dict_huf_lens = d_lens;
+        }
+        zxc_seed_kernel<<<1, 32, 0, st>>>(d_dict, E.dict_size, (u32)E.level, (u32*)P.seed_head, (unsigned short*)P.seed_chain);
+        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    }
+    P.src_size = E.src_size;
+    P.scratch_stride = enc_layout(E.block_size, E.level).total;
+    P.block_size = E.block_size;
+    P.n_blocks = E.n_blocks;
+    P.staging_stride = enc_staging_stride(E.block_size);
+    P.level = (u32)E.level;
+    P.checksum = E.checksum ? 1u : 0u;
+    P.dict_size = P.dict ? E.dict_size : 0;
+    if (cudaMemsetAsync(E.counter, 0, sizeof(unsigned long long), st) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    const u32 grid = E.warps >= ENC_WARPS_PER_CTA ? E.warps / ENC_WARPS_PER_CTA : 1u;
+    const u32 threads = E.warps >= ENC_WARPS_PER_CTA ? ENC_CTA_THREADS : 32u * E.warps;
+    if (E.level >= 6) zxc_encode_kernel<true><<<grid, threads, 0, st>>>(P);
+    else zxc_encode_kernel<false><<<grid, threads, 0, st>>>(P);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* gather the staging slots to out + dst_off[j] */
+static void launch_compact(const u8* d_stage, u32 sstride, const unsigned long long* d_offs, const u32* d_sizes,
+                           u8* out, u32 n_blocks, cudaStream_t st) {
+    const u32 cmax = (u32)(g_sm_count > 0 ? g_sm_count : 132) * 8u;
+    const u32 cgrid = (n_blocks + 7) / 8 < cmax ? (n_blocks + 7) / 8 : cmax;
+    zxc_compact_kernel<<<cgrid, 256, 0, st>>>(d_stage, sstride, d_offs, d_sizes, out, n_blocks);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+}
+
 /* Encodes src into the frame BODY (all data blocks back to back) in h_body.  h_sizes receives
  * n_blocks on-disk block sizes.  Returns ZXC_OK, or ZXC_ERROR_DST_TOO_SMALL when the body does
  * not fit body_cap (then *body_size holds the size that would have been needed). */
@@ -1234,61 +1325,25 @@ extern "C" int zxg_encode_body(zxg_ctx* c, const uint8_t* h_src, uint64_t src_si
     if (n_blocks == 0) return ZXC_OK;
     const u32 sstride = enc_staging_stride(block_size);
     const size_t wstride = enc_layout(block_size, level).total;
-    const u32 ctas_needed = (n_blocks + ENC_WARPS_PER_CTA - 1) / ENC_WARPS_PER_CTA;
-    const u32 resident = (u32)(g_sm_count > 0 ? g_sm_count : 132) * ENC_CTAS_PER_SM;
-    const u32 grid = ctas_needed < resident ? ctas_needed : resident;
+    const u32 warps = enc_full_warps(n_blocks);
     u8* d_src = (u8*)zxg_buffer(c, ZXG_BUF_IN, (size_t)src_size + 64);
     u8* d_stage = (u8*)zxg_buffer(c, ZXG_BUF_OUT, (size_t)n_blocks * sstride);
-    u8* d_scratch = (u8*)zxg_buffer(c, ZXG_BUF_SCRATCH, (size_t)grid * ENC_WARPS_PER_CTA * wstride);
+    u8* d_scratch = (u8*)zxg_buffer(c, ZXG_BUF_SCRATCH, (size_t)warps * wstride);
     u32* d_sizes = (u32*)zxg_buffer(c, ZXG_BUF_STATUS, (size_t)n_blocks * 4);
     unsigned long long* d_offs = (unsigned long long*)zxg_buffer(c, ZXG_BUF_JOBS, (size_t)n_blocks * 8);
     if (!d_src || !d_stage || !d_scratch || !d_sizes || !d_offs) return ZXC_ERROR_MEMORY;
     int rc = zxg_h2d(c, d_src, h_src, (size_t)src_size);
     if (rc != ZXC_OK) return rc;
     if (cudaMemsetAsync(d_src + src_size, 0, 64, c->stream) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
-    EncodeParams P;
-    P.src = d_src;
-    P.staging = d_stage;
-    P.out_size = d_sizes;
-    P.scratch = d_scratch;
-    P.counter = c->counter;
-    P.dict = NULL;
-    P.seed_head = NULL;
-    P.seed_chain = NULL;
-    P.dict_huf_lens = NULL;
+    u8* d_dict = NULL;
     if (h_dict && dict_size) {
-        /* dictionary + its seeded tables: [dict (padded)] [head 128 KB] [chain 128 KB] */
-        const size_t dpad = ((size_t)dict_size + 16 + 255) & ~(size_t)255;
-        const size_t dtot = dpad + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2 + 256;
-        u8* d_dict = (u8*)zxg_buffer(c, ZXG_BUF_DICT, dtot);
+        d_dict = (u8*)zxg_buffer(c, ZXG_BUF_DICT, enc_dict_bytes(dict_size));
         if (!d_dict) return ZXC_ERROR_MEMORY;
-        if (cudaMemsetAsync(d_dict, 0, dtot, c->stream) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
-        rc = zxg_h2d(c, d_dict, h_dict, dict_size);
-        if (rc != ZXC_OK) return rc;
-        P.dict = d_dict;
-        P.seed_head = (const u32*)(d_dict + dpad);
-        P.seed_chain = (const unsigned short*)(d_dict + dpad + (size_t)ENC_HASH_SIZE * 4);
-        if (h_dict_huf_lens && level >= 6) { /* the shared literal table, one length per byte */
-            u8* d_lens = d_dict + dpad + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2;
-            rc = zxg_h2d(c, d_lens, h_dict_huf_lens, 256);
-            if (rc != ZXC_OK) return rc;
-            P.dict_huf_lens = d_lens;
-        }
-        zxc_seed_kernel<<<1, 32, 0, c->stream>>>(d_dict, dict_size, (u32)level, (u32*)P.seed_head, (unsigned short*)P.seed_chain);
-        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     }
-    P.src_size = src_size;
-    P.scratch_stride = wstride;
-    P.block_size = block_size;
-    P.n_blocks = n_blocks;
-    P.staging_stride = sstride;
-    P.level = (u32)level;
-    P.checksum = checksum ? 1u : 0u;
-    P.dict_size = P.dict ? dict_size : 0;
-    if (cudaMemsetAsync(c->counter, 0, sizeof(unsigned long long), c->stream) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
-    if (level >= 6) zxc_encode_kernel<true><<<grid, ENC_CTA_THREADS, 0, c->stream>>>(P);
-    else zxc_encode_kernel<false><<<grid, ENC_CTA_THREADS, 0, c->stream>>>(P);
-    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    const EncLaunch E = {d_src, src_size, block_size, n_blocks, level, checksum, d_stage, d_sizes, d_scratch, warps,
+                         c->counter, d_dict, h_dict, dict_size, h_dict_huf_lens};
+    rc = launch_encode(E, c->stream);
+    if (rc != ZXC_OK) return rc;
     if (cudaMemcpyAsync(h_sizes, d_sizes, (size_t)n_blocks * 4, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
         cudaStreamSynchronize(c->stream) != cudaSuccess) {
         fprintf(stderr, "libzxc (CUDA build): encode kernel failed: %s\n", cudaGetErrorString(cudaGetLastError()));
@@ -1310,15 +1365,107 @@ extern "C" int zxg_encode_body(zxg_ctx* c, const uint8_t* h_src, uint64_t src_si
     u8* d_body = (u8*)zxg_buffer(c, ZXG_BUF_AUX, (size_t)acc + 16);
     rc = d_body ? zxg_h2d(c, d_offs, h_offs, (size_t)n_blocks * 8) : ZXC_ERROR_MEMORY;
     if (rc == ZXC_OK) {
-        const u32 cmax = (u32)(g_sm_count > 0 ? g_sm_count : 132) * 8u;
-        const u32 cgrid = (n_blocks + 7) / 8 < cmax ? (n_blocks + 7) / 8 : cmax;
-        zxc_compact_kernel<<<cgrid, 256, 0, c->stream>>>(d_stage, sstride, d_offs, d_sizes, d_body, n_blocks);
-        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+        launch_compact(d_stage, sstride, d_offs, d_sizes, d_body, n_blocks, c->stream);
         rc = zxg_d2h(c, h_body, d_body, (size_t)acc);
         if (rc == ZXC_OK) rc = zxg_sync(c);
     }
     free(h_offs);
     return rc;
+}
+
+/* ------------------------------------------------------------------------- */
+/* device-to-device compress (zxc_b200_compress_device): the encode above,   */
+/* then the frame assembled on the device (zxc_assemble.cuh)                 */
+/* ------------------------------------------------------------------------- */
+/* Scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned):
+ *   AsmState (256) | input copy + 64 zero bytes | dictionary region (with a dictionary) | staging slots |
+ *   sizes (u32 per block) | body offsets (u64 per block) | tile sums (u64 per ASM_TILE blocks) | per-warp encode slots
+ * The caller's input is copied into the scratch (device to device) so the encode kernel gets the aligned, padded
+ * input it assumes (EncodeParams::src) whatever the caller's alignment and allocation end. */
+struct DevEncLayout {
+    size_t in, dict, stage, sizes, offs, tiles, warps, fixed; /* fixed: bytes before the first warp slot + base slack */
+    size_t wstride;
+};
+static size_t r256(size_t v) { return (v + 255) & ~(size_t)255; }
+static DevEncLayout dev_enc_layout(uint64_t src_size, u32 block_size, u32 n_blocks, int level, u32 dict_size) {
+    DevEncLayout L;
+    size_t o = 256;
+    L.in = o;
+    o += r256((size_t)src_size + 64);
+    L.dict = o;
+    if (dict_size) o += r256(enc_dict_bytes(dict_size));
+    L.stage = o;
+    o += (size_t)n_blocks * enc_staging_stride(block_size);
+    L.sizes = o;
+    o += r256((size_t)n_blocks * 4);
+    L.offs = o;
+    o += r256((size_t)n_blocks * 8);
+    L.tiles = o;
+    o += r256(((size_t)n_blocks + ASM_TILE - 1) / ASM_TILE * 8);
+    L.warps = o;
+    L.fixed = o + 256;
+    L.wstride = enc_layout(block_size, level).total;
+    return L;
+}
+
+extern "C" size_t zxg_encode_scratch_bytes(uint64_t src_size, uint32_t block_size, int level, uint32_t n_blocks,
+                                           uint32_t dict_size) {
+    if (zxg_init() != ZXC_OK) return 0;
+    const DevEncLayout L = dev_enc_layout(src_size, block_size, n_blocks, level, dict_size);
+    return L.fixed + (size_t)(n_blocks ? enc_full_warps(n_blocks) : 1u) * L.wstride;
+}
+
+extern "C" int zxg_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint32_t block_size, int level,
+                                   int checksum, uint32_t n_blocks, const void* h_dict, uint32_t dict_size,
+                                   const uint8_t* h_dict_huf_lens, const zxg_frame_bytes_t* fb, void* d_scratch,
+                                   size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    const DevEncLayout L = dev_enc_layout(src_size, block_size, n_blocks, level, dict_size);
+    if (scratch_size < L.fixed + L.wstride) return ZXC_ERROR_MEMORY;
+    const size_t fit = (scratch_size - L.fixed) / L.wstride;
+    const u32 full = n_blocks ? enc_full_warps(n_blocks) : 1u;
+    const u32 warps = fit < full ? (u32)fit : full;
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    AsmState* state = (AsmState*)base;
+    u8* d_dst8 = (u8*)d_dst;
+    AsmFrame F;
+    memcpy(F.header, fb->header, 16);
+    memcpy(F.eof, fb->eof, 8);
+    memcpy(F.sek, fb->sek, 8);
+    memcpy(F.footer, fb->footer, 12);
+    F.src_size = src_size;
+    F.dst_capacity = fb->dst_capacity;
+    F.fixed = fb->fixed;
+    F.n_blocks = n_blocks;
+    F.block_size = block_size;
+    F.staging_stride = enc_staging_stride(block_size);
+    F.checksum = checksum ? 1u : 0u;
+    F.seekable = fb->seekable ? 1u : 0u;
+    if (n_blocks) {
+        u8* d_in = base + L.in;
+        u8* d_stage = base + L.stage;
+        u32* d_sizes = (u32*)(base + L.sizes);
+        unsigned long long* d_offs = (unsigned long long*)(base + L.offs);
+        unsigned long long* d_tiles = (unsigned long long*)(base + L.tiles);
+        const u32 n_tiles = (u32)(((uint64_t)n_blocks + ASM_TILE - 1) / ASM_TILE);
+        if (cudaMemcpyAsync(d_in, d_src, (size_t)src_size, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+            cudaMemsetAsync(d_in + src_size, 0, 64, st) != cudaSuccess)
+            return ZXC_B200_ERROR_CUDA;
+        const EncLaunch E = {d_in, src_size, block_size, n_blocks, level, checksum, d_stage, d_sizes, base + L.warps,
+                             warps, &state->counter, base + L.dict, h_dict, dict_size, h_dict_huf_lens};
+        const int rc = launch_encode(E, st);
+        if (rc != ZXC_OK) return rc;
+        zxc_asm_tile_sums<<<n_tiles, ASM_THREADS, 0, st>>>(d_sizes, n_blocks, d_tiles);
+        zxc_asm_scan_tiles<<<1, ASM_SCAN_THREADS, 0, st>>>(d_tiles, n_tiles, state, F);
+        zxc_asm_blocks<<<n_tiles, ASM_THREADS, 0, st>>>(d_sizes, d_stage, d_tiles, d_offs, state, d_jobs, d_dst8, F);
+        __atomic_add_fetch(&g_launches, 3, __ATOMIC_RELAXED);
+        launch_compact(d_stage, F.staging_stride, d_offs, d_sizes, d_dst8 + 16 /* file header */, n_blocks, st);
+    }
+    zxc_asm_finish<<<1, 1, 0, st>>>(d_dst8, state, F, (long long*)d_result);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 
 /* ------------------------------------------------------------------------- */

@@ -51,6 +51,26 @@ int zxg_encode_body(zxg_ctx* c, const uint8_t* h_src, uint64_t src_size, uint32_
                     int checksum, uint32_t n_blocks, uint8_t* h_body, uint64_t body_cap, uint32_t* h_sizes,
                     uint64_t* body_size, const void* h_dict, uint32_t dict_size, const uint8_t* h_dict_huf_lens);
 
+/* Device-to-device compress (zxc_b200_compress_device).  The host writes the frame's fixed bytes with the
+ * zxc_format.c helpers; the device places them around the body it assembles. */
+typedef struct {
+    uint8_t header[16];    /* file header */
+    uint8_t eof[8];        /* EOF block header */
+    uint8_t sek[8];        /* SEK block header (when seekable) */
+    uint8_t footer[12];    /* footer with a zero hash; the device writes the hash when checksums are on */
+    uint64_t fixed;        /* file header + trailer bytes */
+    uint64_t dst_capacity;
+    int seekable;          /* a SEK table follows the EOF block (seekable and at least one block) */
+} zxg_frame_bytes_t;
+/* scratch for the full resident encode grid (0 without a device) */
+size_t zxg_encode_scratch_bytes(uint64_t src_size, uint32_t block_size, int level, uint32_t n_blocks,
+                                uint32_t dict_size);
+/* enqueues the copy, encode and assembly on `stream`; ZXC_ERROR_MEMORY when the scratch holds less than one warp */
+int zxg_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint32_t block_size, int level,
+                        int checksum, uint32_t n_blocks, const void* h_dict, uint32_t dict_size,
+                        const uint8_t* h_dict_huf_lens, const zxg_frame_bytes_t* fb, void* d_scratch,
+                        size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
+
 /* Device selection for the calling thread (multi-device fork-join in zxc_api.c): current device, device count,
  * cudaSetDevice.  zxg_acquire() hands out a context of the calling thread's current device. */
 int zxg_current_device(void);

@@ -1,0 +1,148 @@
+"""Device-resident compress / decompress of torch CUDA tensors.
+
+``compress`` runs zxc_b200_compress_device: the frame is encoded and assembled in HBM on a CUDA stream, with no copy
+through the host.  ``decompress`` decodes such a frame with zxc_b200_decode_blocks from the decode plan the
+compress call emitted.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
+"""
+import ctypes as C
+from dataclasses import dataclass
+
+import torch
+
+from . import lib
+
+BLOCK_SIZE_DEFAULT = 512 * 1024
+JOB_BYTES = 24  # zxc_b200_job_t
+
+
+class _Opts(C.Structure):  # zxc_compress_opts_t (include/zxc_opts.h)
+    _fields_ = [("n_threads", C.c_int), ("level", C.c_int), ("block_size", C.c_size_t),
+                ("checksum_enabled", C.c_int), ("seekable", C.c_int), ("dict", C.c_void_p),
+                ("dict_size", C.c_size_t), ("dict_huf", C.c_void_p), ("progress_cb", C.c_void_p),
+                ("user_data", C.c_void_p)]
+
+
+lib.zxc_compress_bound.restype = C.c_uint64
+lib.zxc_compress_bound.argtypes = [C.c_size_t]
+lib.zxc_error_name.restype = C.c_char_p
+lib.zxc_error_name.argtypes = [C.c_int]
+lib.zxc_b200_encode_scratch_size.restype = C.c_size_t
+lib.zxc_b200_encode_scratch_size.argtypes = [C.c_uint64, C.c_void_p]
+lib.zxc_b200_compress_device.restype = C.c_int
+lib.zxc_b200_compress_device.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                         C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]
+lib.zxc_b200_decode_scratch_size.restype = C.c_size_t
+lib.zxc_b200_decode_scratch_size.argtypes = [C.c_uint32]
+lib.zxc_b200_decode_blocks.restype = C.c_int
+lib.zxc_b200_decode_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                       C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_int,
+                                       C.c_void_p]
+lib.zxc_b200_reduce_status.restype = C.c_int64
+lib.zxc_b200_reduce_status.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+
+
+class ZxcError(RuntimeError):
+    def __init__(self, code, what):
+        super().__init__(f"{what}: {lib.zxc_error_name(int(code)).decode()} ({int(code)})")
+        self.code = int(code)
+
+
+@dataclass
+class DeviceFrame:
+    frame: torch.Tensor  # uint8, the complete frame (a view of the compress buffer, trimmed to the frame size)
+    jobs: torch.Tensor  # uint8, n_blocks zxc_b200_job_t: the frame's decode plan
+    block_size: int
+    decoded_size: int
+    checksum: bool
+    dict: bytes = None  # the dictionary the frame needs (host bytes), or None
+    dict_huf: bytes = None
+
+    @property
+    def n_blocks(self):
+        return self.jobs.numel() // JOB_BYTES
+
+
+def _bytes_view(t):
+    if not t.is_cuda:
+        raise ValueError("src must be a CUDA tensor")
+    if not t.is_contiguous():
+        raise ValueError("src must be contiguous")
+    return t.reshape(-1).view(torch.uint8)
+
+
+def compress(src, *, level=0, block_size=0, checksum=False, seekable=False, dict=None, dict_huf=None, stream=None):
+    """Compress a contiguous CUDA tensor (its bytes) into a ZXC frame on its device; returns a DeviceFrame.
+
+    Runs on `stream` (default: torch's current stream of src's device) and synchronises it once to read the frame
+    size.  The frame equals what zxc_compress returns for the same bytes and options."""
+    b = _bytes_view(src)
+    n = b.numel()
+    bs = block_size or BLOCK_SIZE_DEFAULT
+    keep = []
+    o = _Opts(level=level, block_size=block_size, checksum_enabled=int(bool(checksum)), seekable=int(bool(seekable)))
+    if dict is not None:
+        d = bytes(dict)
+        keep.append(d)
+        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+        if dict_huf is not None:
+            h = bytes(dict_huf)
+            keep.append(h)
+            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    with torch.cuda.device(b.device):
+        stream = stream or torch.cuda.current_stream(b.device)
+        with torch.cuda.stream(stream):
+            scratch_size = int(lib.zxc_b200_encode_scratch_size(n, C.byref(o)))
+            if scratch_size == 0:
+                raise ValueError("zxc_b200_encode_scratch_size: invalid options (level, block_size, dict) or no device")
+            cap = int(lib.zxc_compress_bound(n))
+            dst = torch.empty(cap, dtype=torch.uint8, device=b.device)
+            scratch = torch.empty(scratch_size, dtype=torch.uint8, device=b.device)
+            result = torch.empty(1, dtype=torch.int64, device=b.device)
+            n_blocks = (n + bs - 1) // bs
+            jobs = torch.empty(max(n_blocks, 1) * JOB_BYTES, dtype=torch.uint8, device=b.device)[: n_blocks * JOB_BYTES]
+            rc = lib.zxc_b200_compress_device(b.data_ptr() if n else None, n, dst.data_ptr(), cap, C.byref(o),
+                                              scratch.data_ptr(), scratch_size, result.data_ptr(),
+                                              jobs.data_ptr() if n_blocks else None, stream.cuda_stream)
+            if rc != 0:
+                raise ZxcError(rc, "zxc_b200_compress_device")
+            stream.synchronize()
+            size = int(result.item())
+    if size < 0:
+        raise ZxcError(size, "zxc_b200_compress_device")
+    return DeviceFrame(dst[:size], jobs, bs, n, bool(checksum), keep[0] if dict is not None else None,
+                       keep[1] if dict_huf is not None and dict is not None else None)
+
+
+def decompress(f, *, verify=False, stream=None):
+    """Decode a DeviceFrame on its device; returns a uint8 CUDA tensor of f.decoded_size bytes.
+
+    Runs zxc_b200_decode_blocks on `stream` (default: torch's current stream) and zxc_b200_reduce_status, which
+    synchronises it.  verify=True checks the block checksums (the frame must carry them)."""
+    dev = f.frame.device
+    with torch.cuda.device(dev):
+        stream = stream or torch.cuda.current_stream(dev)
+        with torch.cuda.stream(stream):
+            out = torch.empty(f.decoded_size, dtype=torch.uint8, device=dev)
+            n = f.n_blocks
+            if n == 0:
+                return out
+            status = torch.empty(n, dtype=torch.int32, device=dev)
+            scratch_size = int(lib.zxc_b200_decode_scratch_size(f.block_size))
+            scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
+            d_dict = d_huf = None
+            dict_size = 0
+            if f.dict is not None:
+                host = f.dict + (f.dict_huf or b"")
+                dd = torch.frombuffer(bytearray(host), dtype=torch.uint8).to(dev)
+                d_dict, dict_size = dd.data_ptr(), len(f.dict)
+                d_huf = d_dict + dict_size if f.dict_huf is not None else None
+            rc = lib.zxc_b200_decode_blocks(f.frame.data_ptr(), out.data_ptr(), f.jobs.data_ptr(), n,
+                                            status.data_ptr(), d_dict, dict_size, d_huf, scratch.data_ptr(),
+                                            scratch_size, f.block_size, int(bool(verify and f.checksum)),
+                                            stream.cuda_stream)
+            if rc != 0:
+                raise ZxcError(rc, "zxc_b200_decode_blocks")
+            r = int(lib.zxc_b200_reduce_status(status.data_ptr(), f.jobs.data_ptr(), n, stream.cuda_stream))
+    if r != f.decoded_size:
+        raise ZxcError(r if r < 0 else -8, "zxc_b200_decode_blocks")
+    return out
