@@ -93,7 +93,8 @@ ZXC_EXPORT size_t zxc_b200_encode_scratch_size(uint64_t src_size, const zxc_comp
 
 /* Compress src_size bytes at d_src into a complete ZXC frame at d_dst, on `stream`, asynchronously.
  *   opts       as for zxc_compress: level, block_size, checksum_enabled, seekable, and dict / dict_size /
- *              dict_huf in HOST memory (the dictionary is read before the call returns)
+ *              dict_huf in HOST memory, pageable or page-locked (the dictionary has been read when the call
+ *              returns: it is staged through a pageable host copy)
  *   d_scratch  device scratch; with less than zxc_b200_encode_scratch_size(...) bytes the encode runs as many
  *              warps as the scratch holds (same output, slower); below one warp's worth the call fails
  *   d_result   one device int64: the frame size, or ZXC_ERROR_DST_TOO_SMALL when the frame does not fit
@@ -113,6 +114,54 @@ ZXC_EXPORT size_t zxc_b200_encode_scratch_size(uint64_t src_size, const zxc_comp
 ZXC_EXPORT int zxc_b200_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
                                         const zxc_compress_opts_t* opts, void* d_scratch, size_t scratch_size,
                                         int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
+
+/* Device scratch for zxc_b200_decompress_device: frames whose file-header block size is at most block_size,
+ * decoded into at most dst_capacity bytes (0: bad block size, or no device).  It holds a job table of
+ * J = ceil(dst_capacity / ZXC_BLOCK_SIZE_MIN) + 2 entries and the decode kernels' per-warp scratch for block_size;
+ * on an H100 (132 SMs), 4 GiB of output takes 150 MiB at 4 KiB blocks and 935 MiB at 64 KiB blocks. */
+ZXC_EXPORT size_t zxc_b200_decompress_device_scratch_size(uint64_t dst_capacity, uint32_t block_size);
+
+/* Decompress the frame at d_src[0 .. src_size) into d_dst, on `stream`, asynchronously.
+ * *d_result (one device int64) becomes exactly what zxc_decompress returns for the same bytes, capacity and opts,
+ * and d_dst[0 .. *d_result) equals its output.
+ *   opts       as for zxc_decompress: checksum_enabled, and dict / dict_size / dict_huf in HOST memory, pageable or
+ *              page-locked (the dictionary has been read when the call returns: it is staged through a pageable
+ *              host copy, then copied into the scratch; a call with a dictionary allocates that host copy, may wait
+ *              for the stream, and cannot be captured in a CUDA graph)
+ *   d_scratch  at least zxc_b200_decompress_device_scratch_size(dst_capacity, B) bytes for some block size B; frames
+ *              with blocks larger than the largest such B get ZXC_ERROR_MEMORY in *d_result
+ * Returns ZXC_OK once enqueued, or what the host decides without reading the frame, in zxc_decompress's order:
+ * ZXC_ERROR_NULL_INPUT (also for a NULL d_scratch or d_result, or a NULL d_dst with dst_capacity > 0),
+ * ZXC_ERROR_SRC_TOO_SMALL (src_size below file header + footer), ZXC_ERROR_DICT_TOO_LARGE, ZXC_B200_ERROR_NO_DEVICE,
+ * then ZXC_ERROR_MEMORY when the scratch is smaller than zxc_b200_decompress_device_scratch_size(dst_capacity, 4096).
+ * The device decides everything that depends on the frame's bytes, in zxc_decompress's order, and writes it to
+ * *d_result: the dst_capacity == 0 shortcut (magic, then footer), the file-header rejects, DICT_REQUIRED /
+ * DICT_MISMATCH against the header's dictionary id and a malformed dict_huf, the first failing block, capacity,
+ * BAD_HEADER at the end of the block stream, the footer size, and the global hash (checked when
+ * opts->checksum_enabled and the frame has checksums).  Two limits of this call also give ZXC_ERROR_MEMORY there:
+ *   - a header block size larger than the scratch was sized for (decided right after the file-header checks);
+ *   - a frame that needs the general re-plan with more blocks ahead of its end than the job table's J entries.  The
+ *     re-plan runs when the regular plan (block i at i * block_size) fails with a size mismatch -- a block that
+ *     decodes to another size than planned, or runs out of room -- or when blocks do not fit dst_capacity while the
+ *     footer's size does.  zxc_decompress then gives a block's error, DST_TOO_SMALL or a size, this call gives
+ *     ZXC_ERROR_MEMORY when the frame has more than J blocks.  That takes hand-stitched frames of many short blocks,
+ *     or a frame with more than J blocks whose footer was damaged down to at most dst_capacity; a frame the
+ *     reference's encoder writes, undamaged, never needs the re-plan.
+ * Nothing outside d_dst[0 .. dst_capacity), the scratch and *d_result is written.  Reads of the frame: the planner
+ * reads d_src[0 .. src_size) byte by byte, so d_src may have any alignment.  The decode kernels (those of
+ * zxc_b200_decode_blocks) copy literal runs with aligned 4-byte loads that reach at most 6 bytes before and 8 bytes
+ * past a run.  In a frame that ends with its EOF block and footer every run lies at least 20 bytes before the end,
+ * so those loads stay inside d_src[0 .. src_size).  Only a truncated frame, whose last block runs to src_size, may
+ * have up to 8 bytes behind d_src + src_size read: keep 8 readable bytes there when frames come from an untrusted
+ * source.  d_src and d_dst must not overlap (in-place decode is zxc_decompress_inplace).  Without a dictionary the call makes no host synchronisation and no allocation and may be
+ * captured in a CUDA graph.  Kernel launches per call (zxc_b200_launch_count): 12 + k * (2 + c), where k is the
+ * number of block sizes from 4 KiB up to B (B = 64 KiB: k = 5) and c = 1 when opts->checksum_enabled, else 0.  The
+ * frame is planned on the device (a parallel plan from its SEK table when it has one, else a sequential walk of its
+ * block headers), decoded by the same kernels as zxc_b200_decode_blocks, and, for frames whose non-final blocks
+ * decode to less than block_size, re-planned and decoded again at the true offsets (see DESIGN.md). */
+ZXC_EXPORT int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                                          const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                                          int64_t* d_result, void* stream);
 
 /* Kernels launched by this library since load (for bench.py's gpu_launches). */
 ZXC_EXPORT uint64_t zxc_b200_launch_count(void);

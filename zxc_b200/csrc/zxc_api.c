@@ -952,6 +952,31 @@ int zxc_b200_compress_device(const void* d_src, uint64_t src_size, void* d_dst, 
                                d_jobs, stream);
 }
 
+size_t zxc_b200_decompress_device_scratch_size(uint64_t dst_capacity, uint32_t block_size) {
+    if (!zxf_valid_block_size(block_size)) return 0;
+    return zxg_decompress_scratch_bytes(dst_capacity, block_size);
+}
+
+/* The host decides what needs no frame bytes, in zxc_decompress's order (decompress_entry, decompress_frame); the
+ * device decides the rest and writes it to *d_result (zxc_dplan.cuh). */
+int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                               const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                               int64_t* d_result, void* stream) {
+    if (!d_src || (!d_dst && dst_capacity != 0) || !d_scratch || !d_result) return ZXC_ERROR_NULL_INPUT;
+    if (src_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE) return ZXC_ERROR_SRC_TOO_SMALL;
+    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
+    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
+    const int arc = dict_size ? dict_huf_attach(dict_huf) : 0;
+    return zxg_decompress_device(d_src, src_size, d_dst, dst_capacity, dict_size ? dict : NULL, (uint32_t)dict_size,
+                                 arc == 1 ? dict_huf : NULL, did, arc, opts ? opts->checksum_enabled : 0, d_scratch,
+                                 scratch_size, d_result, stream);
+}
+
 int64_t zxc_compress_cctx(zxc_cctx* cctx, const void* src, size_t src_size, void* dst, size_t dst_capacity,
                           const zxc_compress_opts_t* opts) {
     if (!cctx) return ZXC_ERROR_NULL_INPUT;

@@ -29,6 +29,7 @@
 #include "zxc_decode2.cuh"
 #include "zxc_encode.cuh"
 #include "zxc_assemble.cuh"
+#include "zxc_dplan.cuh"
 #include "zxc_train.cuh"
 
 /* ========================================================================= */
@@ -652,11 +653,12 @@ extern "C" size_t zxc_b200_decode_scratch_size(uint32_t block_size) {
     return n + (size_t)DEFER_CAP * 4 + SCRATCH_TAIL;
 }
 
-/* d_counter: two 64-bit work counters (zeroed here) */
-static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d_jobs, u32 n_jobs,
-                         i32* d_status, const void* d_dict, u32 dict_size, const void* d_dict_huf,
-                         void* d_scratch, size_t scratch_size, u32 block_size, int verify,
-                         unsigned long long* d_counter, cudaStream_t st) {
+/* d_counter: three 64-bit work counters, zeroed here unless `preset` (then the caller has set them already: the
+ * device-planned decode starts the claims at its first real job, zxc_dplan.cuh) */
+static int launch_decode_ex(const void* d_src, void* d_dst, const zxc_b200_job_t* d_jobs, u32 n_jobs,
+                            i32* d_status, const void* d_dict, u32 dict_size, const void* d_dict_huf,
+                            void* d_scratch, size_t scratch_size, u32 block_size, int verify,
+                            unsigned long long* d_counter, cudaStream_t st, int preset) {
     if (n_jobs == 0) return ZXC_OK;
     DecodeParams P;
     P.src = (const u8*)d_src;
@@ -689,7 +691,8 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
     const int grid = grid_for(n_jobs);
     const size_t warp_scratch = (size_t)grid * WARPS_PER_CTA * P.scratch_stride;
     if (warp_scratch > scratch_size) return ZXC_ERROR_MEMORY;
-    if (cudaMemsetAsync(d_counter, 0, 3 * sizeof(unsigned long long), st) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    if (!preset && cudaMemsetAsync(d_counter, 0, 3 * sizeof(unsigned long long), st) != cudaSuccess)
+        return ZXC_B200_ERROR_CUDA;
     /* deferred-job list behind the per-warp scratch (and the block-cooperative kernel's spill area); its counter is the
      * third work counter.  A scratch too small for it leaves the list empty: the second launch scans the status array. */
     size_t off = (warp_scratch + 255) & ~(size_t)255;
@@ -808,6 +811,14 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
     }
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d_jobs, u32 n_jobs,
+                         i32* d_status, const void* d_dict, u32 dict_size, const void* d_dict_huf,
+                         void* d_scratch, size_t scratch_size, u32 block_size, int verify,
+                         unsigned long long* d_counter, cudaStream_t st) {
+    return launch_decode_ex(d_src, d_dst, d_jobs, n_jobs, d_status, d_dict, dict_size, d_dict_huf, d_scratch,
+                            scratch_size, block_size, verify, d_counter, st, 0);
 }
 
 /* device scratch one launch over n_jobs blocks needs (without the counter tail) */
@@ -1382,6 +1393,16 @@ extern "C" int zxg_encode_body(zxg_ctx* c, const uint8_t* h_src, uint64_t src_si
  *   sizes (u32 per block) | body offsets (u64 per block) | tile sums (u64 per ASM_TILE blocks) | per-warp encode slots
  * The caller's input is copied into the scratch (device to device) so the encode kernel gets the aligned, padded
  * input it assumes (EncodeParams::src) whatever the caller's alignment and allocation end. */
+/* A copy of n host bytes (of a buffer of `bytes`) in fresh pageable memory.  cudaMemcpyAsync from pageable memory
+ * returns only once it has read the source (it stages it for the DMA), while from page-locked memory it returns before
+ * the copy runs: the device-to-device calls promise to have read the caller's dictionary when they return, so a
+ * caller may reuse even a pinned one at once.  NULL on allocation failure; the caller frees it after the copy call. */
+static void* host_bounce(const void* p, size_t n, size_t bytes) {
+    void* b = malloc(bytes);
+    if (b) memcpy(b, p, n);
+    return b;
+}
+
 struct DevEncLayout {
     size_t in, dict, stage, sizes, offs, tiles, warps, fixed; /* fixed: bytes before the first warp slot + base slack */
     size_t wstride;
@@ -1453,9 +1474,13 @@ extern "C" int zxg_compress_device(const void* d_src, uint64_t src_size, void* d
         if (cudaMemcpyAsync(d_in, d_src, (size_t)src_size, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
             cudaMemsetAsync(d_in + src_size, 0, 64, st) != cudaSuccess)
             return ZXC_B200_ERROR_CUDA;
+        /* the dictionary is read before the call returns, whatever memory the caller's is in (host_bounce) */
+        void* bd = NULL;
+        if (h_dict && dict_size && !(bd = host_bounce(h_dict, dict_size, dict_size))) return ZXC_ERROR_MEMORY;
         const EncLaunch E = {d_in, src_size, block_size, n_blocks, level, checksum, d_stage, d_sizes, base + L.warps,
-                             warps, &state->counter, base + L.dict, h_dict, dict_size, h_dict_huf_lens};
+                             warps, &state->counter, base + L.dict, bd, dict_size, h_dict_huf_lens};
         const int rc = launch_encode(E, st);
+        free(bd);
         if (rc != ZXC_OK) return rc;
         zxc_asm_tile_sums<<<n_tiles, ASM_THREADS, 0, st>>>(d_sizes, n_blocks, d_tiles);
         zxc_asm_scan_tiles<<<1, ASM_SCAN_THREADS, 0, st>>>(d_tiles, n_tiles, state, F);
@@ -1465,6 +1490,161 @@ extern "C" int zxg_compress_device(const void* d_src, uint64_t src_size, void* d
     }
     zxc_asm_finish<<<1, 1, 0, st>>>(d_dst8, state, F, (long long*)d_result);
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* device-to-device decompress (zxc_b200_decompress_device): the frame walk, */
+/* the decode and the verdict on the device (zxc_dplan.cuh)                  */
+/* ------------------------------------------------------------------------- */
+/* Scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned):
+ *   DPlanState | dictionary + its literal table | plan (J jobs) | decode jobs (J) | status (J x i32) |
+ *   split sizes (J x i32) | SEK tile sums | split probe slots | decode scratch (per-warp regions, deferred list)
+ * J = ceil(dst_capacity / ZXC_BLOCK_SIZE_MIN) + 2: every block but the last of a frame the reference's encoder
+ * writes holds block_size >= ZXC_BLOCK_SIZE_MIN bytes, so such a frame fits the table when its output fits
+ * dst_capacity. */
+struct DevDecLayout {
+    size_t dict, plan, jobs, status, sizes, tiles, slots, dec, dec_bytes, total;
+    u32 J, probe_warps, room;
+};
+static bool dev_dec_layout(uint64_t dst_capacity, u32 block_size, DevDecLayout* L) {
+    const uint64_t J64 = dst_capacity / ZXC_BLOCK_SIZE_MIN + (dst_capacity % ZXC_BLOCK_SIZE_MIN != 0) + 2;
+    if (J64 > 0x7FFFFFFFull) return false;
+    const u32 J = (u32)J64;
+    size_t o = DP_STATE_BYTES;
+    L->dict = o;
+    o += r256((size_t)ZXC_DICT_SIZE_MAX + ZXC_HUF_TABLE_SIZE);
+    L->plan = o;
+    o += r256((size_t)J * sizeof(zxc_b200_job_t));
+    L->jobs = o;
+    o += r256((size_t)J * sizeof(zxc_b200_job_t));
+    L->status = o;
+    o += r256((size_t)J * 4);
+    L->sizes = o;
+    o += r256((size_t)J * 4);
+    L->tiles = o;
+    o += r256(((size_t)J + ASM_TILE - 1) / ASM_TILE * 8);
+    /* the split's size probe: one slot of block_size + ZXF_TAIL_PAD per warp, at most 256 MiB of them (a rare path) */
+    L->room = block_size + ZXF_TAIL_PAD;
+    const u32 dec_warps = (u32)grid_for(J) * WARPS_PER_CTA;
+    const u32 by_room = (u32)(((size_t)256 << 20) / L->room);
+    u32 pw = dec_warps < by_room ? dec_warps : by_room;
+    if (pw > J) pw = J;
+    L->probe_warps = pw ? pw : 1;
+    L->slots = o;
+    o += r256((size_t)L->probe_warps * L->room);
+    L->dec = o;
+    L->dec_bytes = launch_scratch_bytes(J, block_size);
+    o += L->dec_bytes;
+    L->total = o + 256; /* base alignment slack */
+    L->J = J;
+    return true;
+}
+
+extern "C" size_t zxg_decompress_scratch_bytes(uint64_t dst_capacity, uint32_t block_size) {
+    if (zxg_init() != ZXC_OK) return 0;
+    DevDecLayout L;
+    return dev_dec_layout(dst_capacity, block_size, &L) ? L.total : 0;
+}
+
+template <bool HAS_DICT>
+static void launch_dsplit(const DSplitArgs& D, u32 phase, u32 grid, cudaStream_t st) {
+    zxc_dsplit_decode<HAS_DICT><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(D, phase);
+}
+
+extern "C" int zxg_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                                     const void* h_dict, uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id,
+                                     int huf_verdict, int checksum_enabled, void* d_scratch, size_t scratch_size,
+                                     int64_t* d_result, void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    /* the largest block size this scratch was sized for */
+    u32 bs = 0;
+    DevDecLayout L;
+    for (u32 b = ZXC_BLOCK_SIZE_MAX; b >= ZXC_BLOCK_SIZE_MIN; b >>= 1) {
+        if (dev_dec_layout(dst_capacity, b, &L) && L.total <= scratch_size) {
+            bs = b;
+            break;
+        }
+    }
+    if (!bs) return ZXC_ERROR_MEMORY;
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    DPlanState* S = (DPlanState*)base;
+    const bool has_dict = h_dict && dict_size;
+    u8* d_dict = NULL;
+    u8* d_huf = NULL;
+    if (has_dict) { /* read before the call returns, whatever memory the caller's dictionary is in (host_bounce) */
+        d_dict = base + L.dict;
+        const size_t dbytes = (size_t)dict_size + (h_dict_huf ? ZXC_HUF_TABLE_SIZE : 0);
+        u8* b = (u8*)host_bounce(h_dict, dict_size, dbytes);
+        if (!b) return ZXC_ERROR_MEMORY;
+        if (h_dict_huf) {
+            memcpy(b + dict_size, h_dict_huf, ZXC_HUF_TABLE_SIZE);
+            d_huf = d_dict + dict_size;
+        }
+        const cudaError_t e = cudaMemcpyAsync(d_dict, b, dbytes, cudaMemcpyHostToDevice, st);
+        free(b);
+        if (e != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    }
+    DPlanArgs A;
+    A.src = (const u8*)d_src;
+    A.src_size = src_size;
+    A.dst_capacity = dst_capacity;
+    A.plan = (zxc_b200_job_t*)(base + L.plan);
+    A.jobs = (zxc_b200_job_t*)(base + L.jobs);
+    A.status = (i32*)(base + L.status);
+    A.sizes = (i32*)(base + L.sizes);
+    A.tiles = (unsigned long long*)(base + L.tiles);
+    A.st = S;
+    A.result = (long long*)d_result;
+    A.J = L.J;
+    A.max_block_size = bs;
+    A.dict_id = dict_id;
+    A.have_dict = has_dict ? 1u : 0u;
+    A.huf_verdict = huf_verdict;
+    A.checksum_enabled = checksum_enabled ? 1u : 0u;
+    const u32 n_tiles = (L.J + ASM_TILE - 1) / ASM_TILE;
+    const u32 per_job = (L.J + DP_THREADS - 1) / DP_THREADS;
+    zxc_dplan_probe<<<1, 1, 0, st>>>(A);
+    zxc_dplan_sek_tiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dplan_sek_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_dplan_sek_blocks<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dplan_walk<<<1, 32, 0, st>>>(A);
+    zxc_dplan_place<<<per_job, DP_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
+    /* one launch slot per block size up to bs, and per checksum verification off / on; only the frame's has work */
+    u8* dec = base + L.dec;
+    for (u32 b = ZXC_BLOCK_SIZE_MIN; b <= bs; b <<= 1) {
+        const u32 lg = (u32)__builtin_ctz(b) - ZXC_BLOCK_SIZE_MIN_LOG2;
+        for (int v = 0; v <= (checksum_enabled ? 1 : 0); v++) {
+            const int rc = launch_decode_ex(d_src, d_dst, A.jobs, L.J, A.status, d_dict, dict_size, d_huf, dec,
+                                            L.dec_bytes, b, v, S->ctr[lg * 2 + v], st, 1);
+            if (rc != ZXC_OK) return rc;
+        }
+    }
+    zxc_dplan_check<<<per_job, DP_THREADS, 0, st>>>(A);
+    zxc_dplan_decide<<<1, 1, 0, st>>>(A);
+    DSplitArgs D;
+    D.a = A;
+    D.dst = (u8*)d_dst;
+    D.slots = base + L.slots;
+    D.scratch = dec;
+    D.dict = d_dict;
+    D.dict_huf = d_huf;
+    D.dict_size = has_dict ? dict_size : 0;
+    D.scratch_stride = scratch_stride_for(bs);
+    D.room = L.room;
+    D.probe_warps = L.probe_warps;
+    const u32 probe_grid = (L.probe_warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
+    const u32 dec_grid = (u32)grid_for(L.J);
+    if (has_dict) launch_dsplit<true>(D, 0, probe_grid, st);
+    else launch_dsplit<false>(D, 0, probe_grid, st);
+    zxc_dsplit_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    if (has_dict) launch_dsplit<true>(D, 1, dec_grid, st);
+    else launch_dsplit<false>(D, 1, dec_grid, st);
+    zxc_dsplit_final<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 

@@ -71,6 +71,17 @@ int zxg_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint3
                         const uint8_t* h_dict_huf_lens, const zxg_frame_bytes_t* fb, void* d_scratch,
                         size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
 
+/* Device-to-device decompress (zxc_b200_decompress_device).  The host passes what needs no frame bytes: the
+ * dictionary (copied into the scratch), its zxc_dict_id and the dict_huf_attach verdict of its table (h_dict_huf NULL
+ * unless that table is used).  Scratch for frames of at most block_size-byte blocks decoded into dst_capacity bytes
+ * (0 without a device or for a dst_capacity too large to plan); ZXC_ERROR_MEMORY when the scratch holds less than
+ * that for 4 KiB blocks. */
+size_t zxg_decompress_scratch_bytes(uint64_t dst_capacity, uint32_t block_size);
+int zxg_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                          const void* h_dict, uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id,
+                          int huf_verdict, int checksum_enabled, void* d_scratch, size_t scratch_size,
+                          int64_t* d_result, void* stream);
+
 /* Device selection for the calling thread (multi-device fork-join in zxc_api.c): current device, device count,
  * cudaSetDevice.  zxg_acquire() hands out a context of the calling thread's current device. */
 int zxg_current_device(void);

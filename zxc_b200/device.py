@@ -2,7 +2,8 @@
 
 ``compress`` runs zxc_b200_compress_device: the frame is encoded and assembled in HBM on a CUDA stream, with no copy
 through the host.  ``decompress`` decodes such a frame with zxc_b200_decode_blocks from the decode plan the
-compress call emitted.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
+compress call emitted.  ``decompress_frame`` decodes any frame held in a uint8 CUDA tensor with
+zxc_b200_decompress_device, which plans, decodes and checks it on the device.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
 """
 import ctypes as C
 from dataclasses import dataclass
@@ -37,8 +38,19 @@ lib.zxc_b200_decode_blocks.restype = C.c_int
 lib.zxc_b200_decode_blocks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
                                        C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_int,
                                        C.c_void_p]
+lib.zxc_b200_decompress_device_scratch_size.restype = C.c_size_t
+lib.zxc_b200_decompress_device_scratch_size.argtypes = [C.c_uint64, C.c_uint32]
+lib.zxc_b200_decompress_device.restype = C.c_int
+lib.zxc_b200_decompress_device.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                           C.c_size_t, C.c_void_p, C.c_void_p]
 lib.zxc_b200_reduce_status.restype = C.c_int64
 lib.zxc_b200_reduce_status.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+
+
+class _DOpts(C.Structure):  # zxc_decompress_opts_t (include/zxc_opts.h)
+    _fields_ = [("n_threads", C.c_int), ("checksum_enabled", C.c_int), ("dict", C.c_void_p),
+                ("dict_size", C.c_size_t), ("dict_huf", C.c_void_p), ("progress_cb", C.c_void_p),
+                ("user_data", C.c_void_p)]
 
 
 class ZxcError(RuntimeError):
@@ -146,3 +158,62 @@ def decompress(f, *, verify=False, stream=None):
     if r != f.decoded_size:
         raise ZxcError(r if r < 0 else -8, "zxc_b200_decode_blocks")
     return out
+
+
+def decompress_frame(frame, *, capacity=None, dict=None, dict_huf=None, checksum=False, stream=None):
+    """Decode the ZXC frame held in a contiguous uint8 CUDA tensor; returns a uint8 tensor of the decoded bytes.
+
+    Runs zxc_b200_decompress_device on `stream` (default: torch's current stream of the frame's device): the frame is
+    planned, decoded and checked on the device, and the stream is synchronised once to read the result.  The result
+    and the bytes are what zxc_decompress returns for the same frame, capacity and options; an error raises ZxcError
+    with its exact code.  capacity=None reads the decoded size from the frame's 8-byte footer with one small
+    device-to-host copy (together with the header byte that sizes the scratch) and allocates that much output and the
+    scratch for it.  The footer is trusted only as far as zxc_get_decompressed_size trusts it (at most one block of
+    block_size per 8 bytes of frame); a footer past that raises ValueError, and a large plausible one can still ask
+    for more device memory than there is (torch's OutOfMemoryError).  For frames from an untrusted source pass
+    capacity: the output room to allow.  checksum=True verifies the block
+    checksums and the global hash when the frame has them.  dict / dict_huf are host bytes."""
+    if not frame.is_cuda or frame.dtype != torch.uint8 or not frame.is_contiguous():
+        raise ValueError("frame must be a contiguous uint8 CUDA tensor")
+    f = frame.reshape(-1)
+    n = f.numel()
+    o = _DOpts(checksum_enabled=int(bool(checksum)))
+    keep = []
+    if dict is not None:
+        d = bytes(dict)
+        keep.append(d)
+        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+        if dict_huf is not None:
+            h = bytes(dict_huf)
+            keep.append(h)
+            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    dev = f.device
+    with torch.cuda.device(dev):
+        stream = stream or torch.cuda.current_stream(dev)
+        with torch.cuda.stream(stream):
+            # one small copy: the header's block-size code sizes the scratch, the footer gives the default capacity
+            bs, footer = 4096, 0
+            if n >= 28:
+                h = torch.cat([f[5:6], f[n - 12:n - 4]]).cpu().numpy().tobytes()
+                bs, footer = 1 << h[0] if 12 <= h[0] <= 21 else 4096, int.from_bytes(h[1:], "little")
+            if capacity is None:
+                if -(-footer // bs) > n // 8:  # zxf_dsize_plausible: more blocks than the frame has room for
+                    raise ValueError(f"the frame's footer claims {footer} bytes, more than it can hold; pass capacity")
+                capacity = footer
+            capacity = int(capacity)
+            scratch_size = int(lib.zxc_b200_decompress_device_scratch_size(capacity, bs))
+            if scratch_size == 0:
+                raise ValueError("zxc_b200_decompress_device_scratch_size: capacity too large, or no device")
+            out = torch.empty(max(capacity, 1), dtype=torch.uint8, device=dev)
+            scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
+            result = torch.empty(1, dtype=torch.int64, device=dev)
+            rc = lib.zxc_b200_decompress_device(f.data_ptr(), n, out.data_ptr() if capacity else None, capacity,
+                                                C.byref(o), scratch.data_ptr(), scratch_size, result.data_ptr(),
+                                                stream.cuda_stream)
+            if rc != 0:
+                raise ZxcError(rc, "zxc_b200_decompress_device")
+            stream.synchronize()
+            r = int(result.item())
+    if r < 0:
+        raise ZxcError(r, "zxc_b200_decompress_device")
+    return out[:r]
