@@ -166,6 +166,10 @@ ZXC_EXPORT int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, 
 /* Kernels launched by this library since load (for bench.py's gpu_launches). */
 ZXC_EXPORT uint64_t zxc_b200_launch_count(void);
 
+/* Resident CTAs per SM that the occupancy calculator gives the lean and the general block-decode kernel (dictionary-free
+ * instances) at the dynamic shared memory they launch with, for profiles/occupancy_probe.py.  0 on success. */
+ZXC_EXPORT int zxc_b200_decode_occupancy(int* lean, int* general);
+
 /* Phase times (ms) of the calling thread's last dictionary-training calls, for profiles/train_bench.py: upload,
  * count, segments, host sort, pick (zxc_train_dict); slice upload, histogram encode, code lengths
  * (zxc_train_dict_huf).  Writes min(n, 8) entries and returns their number. */

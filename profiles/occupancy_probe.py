@@ -1,4 +1,4 @@
-"""Occupancy probe of the lean decode kernel: which costs an eighth CTA per SM, the spills or the carve-out step?
+"""Occupancy probe of the lean decode kernel: what the eighth CTA per SM gains, and what the carve-out step costs.
 
 Builds library variants with `make NVEXTRA=... OUT=<dir>` and times each on the frame bench.py measures (Silesia-shaped,
 64 KiB blocks, level 3, seed 1), decode-only through zxc_b200_decode_blocks, the variants alternated round by round so
@@ -7,7 +7,7 @@ its GB/s per round, the spread, and the card's name, power limit and SM clock, r
 
     python profiles/occupancy_probe.py                      # builds every variant into a temporary directory
     python profiles/occupancy_probe.py --out DIR            # builds into DIR (reused when already there)
-    python profiles/occupancy_probe.py --only parent,cta8   # a subset
+    python profiles/occupancy_probe.py --only parent,cta7   # a subset
 
 Needs oracle/_ref/libzxc_ref.so (to compress the frame) and one GPU for the timing; `--build-only` needs neither.
 """
@@ -31,19 +31,17 @@ sys.path.insert(0, ROOT)
 # (130 KB) rounds up to the 132 KB step, where only 7 CTAs of the 64-register build fit.
 # A grid of 7 CTAs per SM (ZXC_B200_DECODE_CTAS=7) of a build that could hold 8 leaves the eighth slot empty: the
 # block scheduler spreads a grid over the SMs breadth-first, and the persistent CTAs never end before the frame does.
+# Each variant's resident CTAs per SM, as the occupancy calculator gives them, are printed beside its timing.
 # name, build (a directory per NVEXTRA), NVEXTRA, environment, what it isolates
 VARIANTS = [
-    ("parent", "parent", "", {}, "baseline: lean at 7 CTAs, 72 registers"),
-    ("pad7", "pad7", "-DLEAN_SMEM_PAD=2048u", {}, "7 CTAs, 164 KB carve-out: the L1 shrink alone"),
-    ("reg64_7", "reg64_7", "-DLEAN_CTAS_PER_SM=8u -DLEAN_CARVEOUT=57", {},
-     "64-register build, 132 KB carve-out hint, so 7 CTAs if the driver follows the hint: the spills alone"),
-    ("cta8", "cta8", "-DLEAN_CTAS_PER_SM=8u", {}, "8 CTAs, 64 registers, 164 KB carve-out: both"),
-    ("cta8_grid7", "cta8", "-DLEAN_CTAS_PER_SM=8u", {"ZXC_B200_DECODE_CTAS": "7"},
-     "the 8-CTA build with a 7-CTA grid: spills and the L1 shrink, without the eighth CTA"),
-    ("parent_grid6", "parent", "", {"ZXC_B200_DECODE_CTAS": "6"}, "the lean instance's own 6 -> 7 CTA step"),
-    ("ring2k_7", "ring2k_7", "-DRING_BYTES=2048u", {}, "7 CTAs, 2 KiB rings"),
-    ("ring2k_8", "ring2k_8", "-DRING_BYTES=2048u -DLEAN_CTAS_PER_SM=8u", {},
-     "8 CTAs, 2 KiB rings: more warps at a 100 KB carve-out"),
+    ("parent", "parent", "", {}, "shipped: lean at 8 CTAs, 64 registers without spills"),
+    ("cta7", "cta7", "-DLEAN_CTAS_PER_SM=7u", {}, "the same source built for 7 CTAs (72 registers)"),
+    ("grid7", "parent", "", {"ZXC_B200_DECODE_CTAS": "7"},
+     "the shipped build with a 7-CTA grid: the eighth CTA alone, at the 164 KB carve-out"),
+    ("pad7", "pad7", "-DLEAN_CTAS_PER_SM=7u -DLEAN_SMEM_PAD=2048u", {},
+     "7 CTAs, 164 KB carve-out: the L1 shrink alone"),
+    ("ring2k_7", "ring2k_7", "-DRING_BYTES=2048u -DLEAN_CTAS_PER_SM=7u", {}, "7 CTAs, 2 KiB rings"),
+    ("ring2k_8", "ring2k_8", "-DRING_BYTES=2048u", {}, "8 CTAs, 2 KiB rings: more warps at a 100 KB carve-out"),
 ]
 LEAN = "_Z17zxc_decode_kernelILb0ELb0ELb0ELb1EEv12DecodeParams"
 
@@ -87,6 +85,9 @@ class Runner:
         self.scratch_size = lib.zxc_b200_decode_scratch_size(bench.BLOCK)
         self.d_scratch = torch.empty(self.scratch_size, dtype=torch.uint8, device=dev)
         self.stream = torch.cuda.current_stream(dev)
+        lean, general = C.c_int(0), C.c_int(0)
+        assert lib.zxc_b200_decode_occupancy(C.byref(lean), C.byref(general)) == 0
+        self.occupancy = (lean.value, general.value)
 
     def step(self):
         d_src, d_dst, d_jobs, d_status = self.bufs
@@ -167,6 +168,7 @@ def main():
             del os.environ[k]
         assert torch.equal(d_dst, want), f"{name}: decoded bytes differ"
         runners[name] = r
+        print(f"{name}: resident CTAs per SM, lean / general instance: {r.occupancy[0]} / {r.occupancy[1]}", flush=True)
     del want
     rates = {v[0]: [] for v in variants}
     for k in range(args.rounds):

@@ -27,6 +27,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "zxc_b200.h"
 #include "zxc_error.h"
 
@@ -69,7 +71,7 @@ typedef int32_t i32;
 #define CTAS_PER_SM 7u            /* register-limited (72 regs x 128 threads); 112 KB of rings, rest is L1 */
 #endif
 #ifndef LEAN_CTAS_PER_SM
-#define LEAN_CTAS_PER_SM CTAS_PER_SM /* the lean instance's own launch bounds (DESIGN.md section 9) */
+#define LEAN_CTAS_PER_SM 8u /* the lean instance's own launch bounds: 64 registers without spills (DESIGN.md section 9) */
 #endif
 #ifndef LEAN_SMEM_PAD
 #define LEAN_SMEM_PAD 0u /* development: extra dynamic shared memory per lean CTA, to move the carve-out step alone */
@@ -104,6 +106,11 @@ struct DecodeParams {
     u32* defer_count; /* ... how many; more than defer_cap means "scan the status array instead" */
     u32 defer_cap;
 };
+
+/* this warp's scratch, past the 256-byte lead-in where word loads may start */
+__host__ __device__ __forceinline__ u8* warp_scratch(const DecodeParams& P, u32 gwarp) {
+    return P.scratch + (size_t)gwarp * P.scratch_stride + 256;
+}
 
 /* ------------------------------------------------------------------------- */
 /* small device helpers                                                      */
@@ -142,9 +149,27 @@ template <int OFF> __device__ __forceinline__ void sts16(u32 a, u32 v) {
 template <int OFF> __device__ __forceinline__ void sts8(u32 a, u32 v) {
     asm volatile("st.shared.u8 [%0+%2], %1;" ::"r"(a), "r"(v), "n"(OFF) : "memory");
 }
+/* v, hidden from the compiler's value tracking: what is derived from it is computed where it is used instead of being
+ * hoisted out of the loop and held in registers across it */
+__device__ __forceinline__ u32 opaque(u32 v) {
+    asm volatile("" : "+r"(v));
+    return v;
+}
+/* generic pointer of shared address a, derived anew at every call */
+__device__ __forceinline__ u8* ring_at(u32 a) { return reinterpret_cast<u8*>(__cvta_shared_to_generic((size_t)opaque(a))); }
+/* the warp's index in the grid, read from the special registers anew at every call */
+__device__ __forceinline__ u32 grid_warp_now() {
+    u32 t, c;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+    asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(c));
+    return c * WARPS_PER_CTA + (t >> 5);
+}
 #else
 extern u8 smem[];
 static inline u32 smem_addr(const void* p) { return (u32)(reinterpret_cast<const u8*>(p) - smem); }
+static inline u32 opaque(u32 v) { return v; }
+static inline u8* ring_at(u32 a) { return smem + a; }
+static inline u32 grid_warp_now() { return blockIdx.x * WARPS_PER_CTA + (threadIdx.x >> 5); }
 template <int OFF> static inline void sts32(u32 a, u32 v) { memcpy(smem + a + OFF, &v, 4); }
 template <int OFF> static inline void sts16(u32 a, u32 v) { const unsigned short h = (unsigned short)v; memcpy(smem + a + OFF, &h, 2); }
 template <int OFF> static inline void sts8(u32 a, u32 v) { smem[a + OFF] = (u8)v; }
@@ -353,7 +378,8 @@ struct Sections {
     u32 enc_off;
 };
 
-/* LEAN: the caller has deferred every block with Huffman literals or tokens, so the PivCo decoder is not compiled in */
+/* LEAN: the caller has deferred every block with Huffman literals or tokens, so the PivCo decoder is not compiled in;
+ * the token section always starts at S.lit + S.n_lit_avail (the decode loop holds no pointer of its own for it) */
 template <bool LEAN>
 __device__ int parse_sections(const u8* pay, u32 comp, bool ghi, u32 cap, const u8* dict_huf, u8* scratch,
                               u32 block_cap, u32 lane, Sections& S) {
@@ -430,6 +456,17 @@ __device__ int parse_sections(const u8* pay, u32 comp, bool ghi, u32 cap, const 
         if (enc_tok != 0 && enc_tok != 2) return ZXC_ERROR_CORRUPT_DATA;
         S.tok = p_data + lit_comp;
         S.offs = S.tok + tok_comp;
+        if (LEAN && S.lit == scratch) {
+            /* RLE literals expanded into the scratch: the tokens and offsets are copied right behind them, short of the
+             * escape-value table; a section that does not fit there (never a valid block) goes to the general instance */
+            const u32 ts = tok_comp + (u32)sz_off;
+            if ((u64)n_lit + ts > scratch_cap + scr_tok_cap(block_cap) + (u32)HUF_WORK_BYTES) return D2_DEFER_STATUS;
+            warp_copy(scratch + n_lit, S.tok, ts, lane);
+            __syncwarp();
+            S.tok = scratch + n_lit;
+        } else if (LEAN && S.n_lit_avail == 0) {
+            S.lit = S.tok; /* RLE section that expands to nothing */
+        }
         if (!LEAN && enc_tok == 2) { /* level 7: Huffman-coded tokens (:1019-1022) */
             /* the reference's token buffer holds block_cap / 5 + 16 sequences (zxc_cctx_max_seq) and its PivCo decoder
              * rejects an empty section; scr_tok_cap(block_cap) >= that + 32 */
@@ -736,10 +773,15 @@ __device__ __forceinline__ void balanced_copy_words(u32 ring_s, u32 m_items, u32
 /* GHI and HAS_DICT are compile-time: the loop below sits at the kernel's register limit, and every branch and live
  * value it does not carry (the other block format's unpack, the dictionary pointer and its source classification)
  * is code the instruction cache does not hold and a register that is not spilled.  LEAN: see decode_job. */
+/* the escape-value table: the rank-table area of a warp's scratch, idle once the sections are parsed */
+__device__ __forceinline__ u32* esc_table(u8* scratch, u32 block_cap) {
+    return reinterpret_cast<u32*>(scratch + scr_lit_cap(block_cap) + scr_tok_cap(block_cap) + (u32)HUF_WORK_BYTES);
+}
+
 template <bool UNITS, bool GHI, bool HAS_DICT, bool LEAN>
 __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const u8* dict_in,
                                u32 dict_size_in, const u8* dict_huf, u8* scratch, u32 scratch_cap, u8* ring,
-                               u32 lane, u32 P_flags) {
+                               u32 lane, const DecodeParams& P) {
     constexpr bool ghi = GHI;
     const u8* dict = HAS_DICT ? dict_in : (const u8*)0;
     const u32 dict_size = HAS_DICT ? dict_size_in : 0u;
@@ -756,7 +798,6 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
 
     /* Output-centric body (zxc_decode_units.cuh): only in the <UNITS = true> instance, which the launch picks on request
      * (ZXC_B200_UNITS=1); the sequence-centric body below is the faster one on every workload measured (DESIGN.md). */
-    (void)P_flags;
     if (UNITS && cap <= 65536u) { /* its tables go where the scratch is idle */
         u8* tok_buf = scratch + scr_lit_cap(scratch_cap);
         u8* hw_area = tok_buf + scr_tok_cap(scratch_cap);
@@ -781,13 +822,18 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
     w.near_lo = 0;
     const u32 ring_s = smem_addr(ring);
     (void)ring_s;
+    /* LEAN: the window's ring pointer is re-derived from ring_s in front of each rare path that uses it */
+#define W_RING()                                     \
+    do {                                             \
+        if constexpr (LEAN) w.ring = ring_at(ring_s); \
+    } while (0)
     u32 O = 0, L = 0, F = 0, epos = 0, ring_lo = 0;
 
     /* Escape values for the whole block up front (segment-map scan over the extras section, zxc_decode2_core.h):
      * a batch then reads its values by ordinal instead of walking the varint chain lane-uniformly.  The values
      * live in the rank-table area of the scratch, idle once the sections are parsed; a section too long for it
      * keeps the per-batch walk. */
-    u32* vals = reinterpret_cast<u32*>(scratch + scr_lit_cap(scratch_cap) + scr_tok_cap(scratch_cap) + (u32)HUF_WORK_BYTES);
+    u32* vals = esc_table(scratch, scratch_cap);
     /* LEAN: an extras section too long for the table goes to the general instance (nothing is written yet), so the
      * batch loop below carries neither the varint cursor nor its walk; without extras every escape reads 0 from the
      * empty table, as the reference reads 0 past the section's end */
@@ -888,14 +934,17 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             }
 #else
             if (!ghi) {
-                a = tok[i];
+                /* LEAN: raw literals, raw tokens and offsets lie one behind the other in the payload, so the loop holds one
+                 * pointer for all three and forms the others from it where they are read */
+                const u8* tk = tok;
+                if constexpr (LEAN) tk = lit + opaque(n_lit_avail);
+                a = tk[i];
 #if ZXC_ALIGNED_LD
                 if (LEAN) {
-                    /* raw tokens: the offsets follow them, so the loop holds no pointer of their own */
                     const u32 oi = n_seq + (enc_off ? i : 2u * i);
-                    if (enc_off) b = (u32)tok[oi];
-                    else if ((reinterpret_cast<uintptr_t>(tok) + n_seq) & 1u) b = ld16(tok + oi);
-                    else b = (u32)*reinterpret_cast<const unsigned short*>(tok + oi);
+                    if (enc_off) b = (u32)tk[oi];
+                    else if ((reinterpret_cast<uintptr_t>(tk) + n_seq) & 1u) b = ld16(tk + oi);
+                    else b = (u32)*reinterpret_cast<const unsigned short*>(tk + oi);
                 } else if (enc_off) b = (u32)offs[i];
                 else if (reinterpret_cast<uintptr_t>(offs) & 1u) b = ld16(offs + 2 * (size_t)i);
                 else b = (u32)reinterpret_cast<const unsigned short*>(offs)[i];
@@ -926,12 +975,15 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
         ZXC_TRACE_MARK(TR_UNPACK, lane);
         u32 k_esc = 0, epos_end = epos;
         if ((m_ll | m_ml) && use_vals) {
+            /* LEAN: the table's address is formed here from the launch parameters, not held across the loop */
+            const u32* vt = vals;
+            if constexpr (LEAN) vt = esc_table(warp_scratch(P, grid_warp_now()), P.block_cap);
             u32 k = ord_base + __popc(m_ll & lt_mask) + __popc(m_ml & lt_mask);
             if (e_ll) {
-                ll += k < n_val ? vals[k] : 0u; /* past the last varint the reference reads 0 (:51-88) */
+                ll += k < n_val ? vt[k] : 0u; /* past the last varint the reference reads 0 (:51-88) */
                 k++;
             }
-            if (e_ml) ml += k < n_val ? vals[k] : 0u;
+            if (e_ml) ml += k < n_val ? vt[k] : 0u;
         } else if (ZXC_RARE((m_ll | m_ml) != 0)) {
             const u32 ord_ll = __popc(m_ll & lt_mask) + __popc(m_ml & lt_mask);
             k_esc = __popc(m_ll) + __popc(m_ml);
@@ -970,6 +1022,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
                 return ZXC_ERROR_BAD_OFFSET;
             }
             __syncwarp();
+            W_RING();
             ring_flush(w, F, O, lane, al16);
             __syncwarp();
             flush_wait(lane);
@@ -982,7 +1035,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             F = O;
             /* re-seed the ring with the last 64 bytes so short sources that straddle O resolve */
             ring_lo = O >= 64 ? O - 64 : 0;
-            for (u32 p = ring_lo + lane; p < O; p += 32) ring[p & mask] = out[p];
+            for (u32 p = ring_lo + lane; p < O; p += 32) w.ring[p & mask] = out[p];
             __syncwarp();
             const u32 q = ((m_ll & 1u) ? 1u : 0u) + ((m_ml & 1u) ? 1u : 0u);
             ord_base += q;
@@ -1035,7 +1088,12 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
                                      : (in_dict || (src_lo >= 8 && src_lo + (i32)ml + 4 <= w.near_lo)));
         const bool m_lane_ok = m_word_ok && ml <= MATCH_SHORT && off >= ml;
         const bool m_grp_ok = m_word_ok && !m_lane_ok && off >= ml; /* chunks of one item run side by side */
-        const u8* m_sp = near ? ring + si : (src_lo < 0 ? dict + ((i32)dict_size + src_lo) : out + src_lo);
+        auto match_src = [&]() -> const u8* {
+            return near ? (LEAN ? ring_at(ring_s + si) : ring + si)
+                        : (src_lo < 0 ? dict + ((i32)dict_size + src_lo) : out + src_lo);
+        };
+        /* LEAN: the source pointer is formed in the match pass, so no 64-bit value of it lives through the literal pass */
+        const u8* m_sp = LEAN ? nullptr : match_src();
         const bool l_word_ok = (out_start & mask) + ll + 4 <= RING_BYTES;
 
         /* ---- dependencies ---- */
@@ -1088,7 +1146,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
                 ready = act && m_free;
                 it_d = mdst;
                 it_n = ml;
-                it_sp = m_sp;
+                it_sp = LEAN ? match_src() : m_sp;
                 lok = m_lane_ok;
                 gok = m_grp_ok;
             }
@@ -1111,8 +1169,9 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
                 m_slow &= m_slow - 1;
                 const u32 d = __shfl_sync(FULL, it_d, j), n = __shfl_sync(FULL, it_n, j);
                 const u32 aux = __shfl_sync(FULL, lit_pass ? lit_start : off, j);
+                W_RING();
                 if (lit_pass) {
-                    for (u32 k = lane; k < n; k += 32) ring[(d + k) & mask] = lit[aux + k];
+                    for (u32 k = lane; k < n; k += 32) w.ring[(d + k) & mask] = lit[aux + k];
                 } else {
                     warp_match_to_ring(w, d, aux, n, lane);
                 }
@@ -1139,6 +1198,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
                     for (u32 k = lane; k < n; k += 32) ring[(d + k) & mask] = ring[(sl + k) & mask];
 #endif
                 } else {
+                    W_RING();
                     warp_match_to_ring(w, d, __shfl_sync(FULL, off, j), n, lane);
                 }
                 __syncwarp();
@@ -1149,6 +1209,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
         /* ---- advance and flush ---- */
         O += T;
         L += TL;
+        W_RING();
         ring_flush(w, F, O & ~511u, lane, al16);
         __syncwarp();
         ZXC_TRACE_MARK(TR_FLUSH, lane);
@@ -1171,6 +1232,8 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
     ST_LIT_CLOSE();
     const u32 rem = n_lit_avail - L;
     if (rem > cap - O) return ZXC_ERROR_OVERFLOW;
+    W_RING();
+#undef W_RING
     ring_flush(w, F, O, lane, al16);
     __syncwarp();
     flush_wait(lane);
@@ -1183,8 +1246,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
  * LEAN: decode only what the bench-shaped frames are made of -- RAW blocks and GLO blocks with raw tokens and raw or
  * RLE literals, in a launch without checksum verification -- and return D2_DEFER_STATUS for every other job, before
  * anything is written to its output; the general instance decodes those.  The lean instance carries neither the PivCo
- * Huffman decoder, the checksum nor the GHI body: a third of the code and a sixth of the spill traffic of the general
- * one (DESIGN.md section 3d). */
+ * Huffman decoder, the checksum nor the GHI body (DESIGN.md section 3d). */
 template <bool UNITS, bool HAS_DICT, bool LEAN = false>
 __device__ int decode_job(const DecodeParams& P, const zxc_b200_job_t& job, u8* scratch, u8* ring, u32 lane) {
     const u8* blk = P.src + job.src_off;
@@ -1207,11 +1269,11 @@ __device__ int decode_job(const DecodeParams& P, const zxc_b200_job_t& job, u8* 
     switch (type) {
         case BT_GLO:
             return decode_lz_block<UNITS, false, HAS_DICT, LEAN>(data, comp, out, job.dst_cap, P.dict, P.dict_size,
-                                                                 P.dict_huf, scratch, P.block_cap, ring, lane, P.flags);
+                                                                 P.dict_huf, scratch, P.block_cap, ring, lane, P);
         case BT_GHI:
             if constexpr (LEAN) return D2_DEFER_STATUS; /* not reached: deferred above */
             else return decode_lz_block<UNITS, true, HAS_DICT, false>(data, comp, out, job.dst_cap, P.dict, P.dict_size,
-                                                                      P.dict_huf, scratch, P.block_cap, ring, lane, P.flags);
+                                                                      P.dict_huf, scratch, P.block_cap, ring, lane, P);
         case BT_RAW:
             if (comp > job.dst_cap) return ZXC_ERROR_DST_TOO_SMALL;
             warp_copy(out, data, comp, lane);
@@ -1224,15 +1286,15 @@ __device__ int decode_job(const DecodeParams& P, const zxc_b200_job_t& job, u8* 
 }
 
 /* LEAN: decode_job<LEAN>; each job it defers is marked D2_DEFER_STATUS and listed for a DEFERRED launch that follows.
- * The lean instance has its own CTAs per SM (LEAN_CTAS_PER_SM), 7 like the general one: at 8 (64 registers) it still
- * spills, and spills cost more than the eighth CTA gains (DESIGN.md section 9). */
+ * The lean instance has its own CTAs per SM (LEAN_CTAS_PER_SM): 8 against the general one's 7, in 64 registers without
+ * spills: it holds no 64-bit ring or token pointer across its loops (ring_at, opaque; DESIGN.md section 9). */
 template <bool UNITS, bool DEFERRED, bool HAS_DICT, bool LEAN>
 __global__ void __launch_bounds__(CTA_THREADS, LEAN ? LEAN_CTAS_PER_SM : CTAS_PER_SM) zxc_decode_kernel(const DecodeParams P) {
     extern __shared__ __align__(16) u8 smem[];
     const u32 lane = threadIdx.x & 31;
     const u32 wic = threadIdx.x >> 5;
     const u32 gwarp = blockIdx.x * WARPS_PER_CTA + wic;
-    u8* scratch = P.scratch + (size_t)gwarp * P.scratch_stride + 256; /* lead-in: word loads may start below */
+    u8* scratch = warp_scratch(P, gwarp);
     u8* ring = smem + (size_t)wic * WARP_SMEM_BYTES;
 #if ZXC_STAGE
     st_init(smem_addr(ring) + RING_BYTES, lane);
@@ -1275,15 +1337,21 @@ __global__ void __launch_bounds__(CTA_THREADS, LEAN ? LEAN_CTAS_PER_SM : CTAS_PE
         }
         return;
     }
+    /* LEAN: the job index in one register (claims end below n_jobs plus one per warp, far below 2^32 for any job table
+     * that fits in device memory), the ring as its shared address */
+    using JobIx = typename std::conditional<LEAN, u32, unsigned long long>::type;
+    u32 ring_s = 0;
+    if constexpr (LEAN) ring_s = smem_addr(ring);
     for (;;) {
         ZXC_TRACE_DECL;
-        unsigned long long j = 0;
-        if (lane == 0) j = atomicAdd(P.counter, 1ull);
-        j = __shfl_sync(FULL, j, 0);
+        unsigned long long c = 0;
+        if (lane == 0) c = atomicAdd(P.counter, 1ull);
+        const JobIx j = __shfl_sync(FULL, (JobIx)c, 0);
         ZXC_TRACE_MARK(TR_CLAIM, lane);
         if (j >= P.n_jobs) break;
         const zxc_b200_job_t job = P.jobs[j];
-        const int r = decode_job<UNITS, HAS_DICT, LEAN>(P, job, scratch, ring, lane);
+        const int r = LEAN ? decode_job<UNITS, HAS_DICT, LEAN>(P, job, warp_scratch(P, grid_warp_now()), ring_at(ring_s), lane)
+                           : decode_job<UNITS, HAS_DICT, LEAN>(P, job, scratch, ring, lane);
         flush_wait(lane); /* nothing of this block is still on its way out of the ring */
         __syncwarp();
         if (lane == 0) {

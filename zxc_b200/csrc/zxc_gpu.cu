@@ -343,6 +343,16 @@ extern "C" int zxc_b200_device_count(void) {
 
 extern "C" uint64_t zxc_b200_launch_count(void) { return g_launches; }
 
+extern "C" int zxc_b200_decode_occupancy(int* lean, int* general) {
+    if (zxg_init() != ZXC_OK) return ZXC_B200_ERROR_CUDA;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(lean, zxc_decode_kernel<false, false, false, true>, CTA_THREADS,
+                                                      DECODE_SMEM_BYTES + LEAN_SMEM_PAD) != cudaSuccess ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(general, zxc_decode_kernel<false, true, false, false>, CTA_THREADS,
+                                                      DECODE_SMEM_BYTES) != cudaSuccess)
+        return ZXC_B200_ERROR_CUDA;
+    return ZXC_OK;
+}
+
 #if ZXC_TRACE
 /* traced build only: copies the current device's phase-trace rows (TRACE_ROWS x TRACE_SLOTS counters) to `host` and
  * zeroes them; returns the number of counters */
@@ -688,7 +698,7 @@ static int launch_decode_ex(const void* d_src, void* d_dst, const zxc_b200_job_t
      * request (ZXC_B200_UNITS=1). */
     const bool units = (P.flags & FLAG_UNITS_ON) != 0;
     P.block_cap = block_size;
-    const int grid = grid_for(n_jobs);
+    int grid = grid_for(n_jobs);
     const size_t warp_scratch = (size_t)grid * WARPS_PER_CTA * P.scratch_stride;
     if (warp_scratch > scratch_size) return ZXC_ERROR_MEMORY;
     if (!preset && cudaMemsetAsync(d_counter, 0, 3 * sizeof(unsigned long long), st) != cudaSuccess)
@@ -798,6 +808,12 @@ static int launch_decode_ex(const void* d_src, void* d_dst, const zxc_b200_job_t
         if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
         P.flags |= FLAG_DEFERRED;
         P.counter = d_counter + 1;
+    }
+    /* the general instances run at CTAS_PER_SM: a grid of the lean instance's size would leave its extra CTAs waiting
+     * for a slot and claiming what is left at the end */
+    {
+        const int resident = (g_sm_count > 0 ? g_sm_count : 132) * (int)CTAS_PER_SM;
+        if (grid > resident) grid = resident;
     }
     if (P.flags & FLAG_DEFERRED) {
         if (has_dict) zxc_decode_kernel<false, true, true, false><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(P);
