@@ -34,7 +34,9 @@ sys.path.insert(0, ROOT)
 # Each variant's resident CTAs per SM, as the occupancy calculator gives them, are printed beside its timing.
 # name, build (a directory per NVEXTRA), NVEXTRA, environment, what it isolates
 VARIANTS = [
-    ("parent", "parent", "", {}, "shipped: lean at 8 CTAs, 64 registers without spills"),
+    ("parent", "parent", "", {}, "shipped: lean at 8 CTAs, 64 registers without spills, look-ahead slot"),
+    ("lookahead0", "lookahead0", "-DZXC_LOOKAHEAD=0", {},
+     "the lean instances without the look-ahead slot (tokens, offsets, escapes loaded at the batch top)"),
     ("cta7", "cta7", "-DLEAN_CTAS_PER_SM=7u", {}, "the same source built for 7 CTAs (72 registers)"),
     ("grid7", "parent", "", {"ZXC_B200_DECODE_CTAS": "7"},
      "the shipped build with a 7-CTA grid: the eighth CTA alone, at the 164 KB carve-out"),

@@ -16,7 +16,8 @@
  *      are recent and from global memory (L2) once flushed.
  * The block format and the presence of a dictionary are template parameters (decode_lz_block<UNITS, GHI, HAS_DICT, LEAN>).
  * The LEAN kernel instance decodes only RAW blocks and GLO blocks with raw or RLE literals and raw tokens, and defers
- * every other block to the general instance (decode_job).
+ * every other block to the general instance (decode_job).  Without a dictionary it reads a batch's tokens, offsets and
+ * first 32 escape values from a per-warp look-ahead slot behind the ring, filled by cp.async while the batch before it copies (ZXC_LOOKAHEAD).
  * zxc_decode_stage.cuh holds the opt-in TMA flavour (sections staged by cp.async.bulk, ring flushed by bulk stores).
  * Overlapping matches (off < ml) use the period-`off` index instead of the reference's shuffle
  * tables (:197-413).  Output is written exactly (no wild-copy overshoot): none of the
@@ -215,6 +216,65 @@ __device__ __forceinline__ void trace_add(u32 slot, unsigned long long v, u32 la
 #include "zxc_decode_stage.cuh"
 #define WARP_SMEM_BYTES (RING_BYTES + STAGE_BYTES) /* a warp's output ring, its staging area right behind */
 #define DECODE_SMEM_BYTES (WARPS_PER_CTA * WARP_SMEM_BYTES)
+
+/* The lean instance without a dictionary stages the next batch's tokens, offsets and escape values into a per-warp look-ahead slot right
+ * behind the ring by cp.async, one batch ahead (DESIGN.md section 3a step 8).  -DZXC_LOOKAHEAD=0 builds it without
+ * the slot, for A/B timing; every other instance is the same either way. */
+#ifndef ZXC_LOOKAHEAD
+#define ZXC_LOOKAHEAD (!ZXC_STAGE)
+#endif
+#if ZXC_LOOKAHEAD && ZXC_STAGE
+#error "ZXC_LOOKAHEAD and ZXC_STAGE both stage the token and offset sections: build with one of them"
+#endif
+#define LA_SLOT_BYTES (ZXC_LOOKAHEAD ? 256u : 0u)
+#define LA_OFF 48u  /* slot bytes [0, 48): token words; [48, 128): offset words */
+#define LA_ESC 128u /* [128, 256): the batch's first 32 escape values */
+#define LEAN_WARP_SMEM_BYTES (WARP_SMEM_BYTES + LA_SLOT_BYTES)
+/* dynamic shared memory of the lean launch without a dictionary; the one with a dictionary has no slot */
+#define LEAN_SMEM_BYTES (WARPS_PER_CTA * LEAN_WARP_SMEM_BYTES + LEAN_SMEM_PAD)
+/* which instance carries the slot: the lean one without a dictionary (with one it measured slower, DESIGN.md 3d) */
+template <bool HAS_DICT, bool LEAN> __host__ __device__ constexpr bool la_on() {
+    return LEAN && !HAS_DICT && ZXC_LOOKAHEAD != 0;
+}
+
+/* 4-byte global -> shared copy that holds no register until it lands; cp_async_wait_all() waits for this thread's */
+#ifdef __CUDACC__
+__device__ __forceinline__ void cp_async4(u32 sdst, const void* gsrc) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(sdst), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_check_idle() {}
+#else
+/* CPU emulator (tests/simt): a copy fills its destination with a poison pattern when it is issued and moves the data
+ * only at the issuing lane's wait, the latest moment the hardware may take.  A read before that lane's wait -- a
+ * missing wait, or a missing __syncwarp() between the other lanes' waits and the read -- sees the poison. */
+struct SimtCpAsync {
+    u32 s;
+    const u8* g;
+};
+inline SimtCpAsync simt_cp_pending[32][8];
+inline u32 simt_cp_n[32];
+static inline void simt_cp_fail(const char* what) {
+    fprintf(stderr, "simt cp.async check failed: %s\n", what);
+    abort();
+}
+static inline void cp_async4(u32 sdst, const void* gsrc) {
+    const int l = simt::g_warp->current;
+    if ((sdst & 3u) || (reinterpret_cast<uintptr_t>(gsrc) & 3u)) simt_cp_fail("4-byte copy not 4-byte aligned");
+    if (simt_cp_n[l] >= 8) simt_cp_fail("more copies in flight than a lane issues per batch");
+    memset(smem + sdst, 0xE7, 4);
+    simt_cp_pending[l][simt_cp_n[l]++] = SimtCpAsync{sdst, static_cast<const u8*>(gsrc)};
+}
+static inline void cp_async_wait_all() {
+    const int l = simt::g_warp->current;
+    for (u32 k = 0; k < simt_cp_n[l]; k++) memcpy(smem + simt_cp_pending[l][k].s, simt_cp_pending[l][k].g, 4);
+    simt_cp_n[l] = 0;
+}
+/* a block starts with no copy of this lane in flight: the previous one waited for all it issued */
+static inline void cp_async_check_idle() {
+    if (simt_cp_n[simt::g_warp->current]) simt_cp_fail("a copy was still in flight when the previous block ended");
+}
+#endif
 
 #include "zxc_huffman.cuh"
 
@@ -778,6 +838,35 @@ __device__ __forceinline__ u32* esc_table(u8* scratch, u32 block_cap) {
     return reinterpret_cast<u32*>(scratch + scr_lit_cap(block_cap) + scr_tok_cap(block_cap) + (u32)HUF_WORK_BYTES);
 }
 
+/* LEAN look-ahead slot (slot_s: LA_SLOT_BYTES of shared memory behind the warp's ring).  Lane l copies slot word l --
+ * a word of the aligned words that cover the tokens of the batch that starts at sequence nb for l < 12, of its
+ * offsets above -- each with one 4-byte cp.async.  tk: the token section, the offsets right behind it.  The words lie
+ * in the sections but for at most 3 bytes either side, which are inside the payload (or the scratch the RLE path
+ * copied the sections to); nothing is copied when no batch follows. */
+__device__ __forceinline__ void la_issue_words(u32 slot_s, const u8* tk, u32 n_seq, u32 enc_off, u32 nb, u32 lane) {
+    if (nb < n_seq) {
+        const u32 nt = min(32u, n_seq - nb), ow = enc_off ? 1u : 2u;
+        const bool t = lane < LA_OFF / 4u;
+        const u8* s = t ? tk + nb : tk + n_seq + ow * nb; /* the batch's first token / offset byte */
+        const u32 n = t ? nt : ow * nt;
+        const u32 x = (u32)reinterpret_cast<uintptr_t>(s) & 3u;
+        const u32 k = t ? lane : lane - LA_OFF / 4u;
+        if (4u * k < x + n) cp_async4(slot_s + 4u * lane, s - x + 4u * k);
+    }
+}
+/* ... and escape value ob + l of the block's table, when there is one */
+__device__ __forceinline__ void la_issue_esc(u32 slot_s, u32 n_val, u32 ob, u32 lane, const DecodeParams& P) {
+    if (ob + lane < n_val)
+        cp_async4(slot_s + LA_ESC + 4u * lane, esc_table(warp_scratch(P, grid_warp_now()), P.block_cap) + ob + lane);
+}
+/* escape value k of a batch whose first ordinal is ob: from the slot for the first 32, else from the table; 0 past
+ * the last varint, as the reference reads (:51-88) */
+__device__ __forceinline__ u32 la_esc(u32 slot_s, u32 k, u32 ob, u32 n_val, const DecodeParams& P) {
+    if (k >= n_val) return 0u;
+    if (k - ob < 32u) return lds32(slot_s + LA_ESC + 4u * (k - ob));
+    return esc_table(warp_scratch(P, grid_warp_now()), P.block_cap)[k];
+}
+
 template <bool UNITS, bool GHI, bool HAS_DICT, bool LEAN>
 __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const u8* dict_in,
                                u32 dict_size_in, const u8* dict_huf, u8* scratch, u32 scratch_cap, u8* ring,
@@ -822,6 +911,11 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
     w.near_lo = 0;
     const u32 ring_s = smem_addr(ring);
     (void)ring_s;
+    /* LEAN: the batch loop reads its tokens, offsets and first escape values from the look-ahead slot, where the
+     * previous batch (or the block start) had them copied */
+    constexpr bool LA = la_on<HAS_DICT, LEAN>();
+    const u32 slot_s = ring_s + WARP_SMEM_BYTES;
+    (void)slot_s;
     /* LEAN: the window's ring pointer is re-derived from ring_s in front of each rare path that uses it */
 #define W_RING()                                     \
     do {                                             \
@@ -839,6 +933,10 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
      * empty table, as the reference reads 0 past the section's end */
     if constexpr (LEAN) {
         if (4ull * ext_end > scr_cum_cap(scratch_cap)) return D2_DEFER_STATUS;
+    }
+    if constexpr (LA) { /* batch 0's tokens and offsets travel during the extras scan, its escape values after it */
+        cp_async_check_idle();
+        la_issue_words(slot_s, tok, n_seq, enc_off, 0u, lane);
     }
     const bool use_vals = LEAN || (ext_end != 0u && 4ull * ext_end <= scr_cum_cap(scratch_cap));
     u32 n_val = 0, ord_base = 0;
@@ -861,6 +959,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
         }
         __syncwarp();
     }
+    if constexpr (LA) la_issue_esc(slot_s, n_val, 0u, lane, P);
 
 #if ZXC_STAGE
     /* the token / offset sections (and raw literals) come through shared memory (zxc_decode_stage.cuh); Huffman-decoded
@@ -897,6 +996,10 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
          * corpus) are requested into L1 now, so that they arrive while the tokens and offsets do and the literal pass
          * finds them there; clamped to the literal section.  (With a dictionary both prefetches measured slower.) */
         if (LEAN && !HAS_DICT && lane < 4u && L + 128u * lane < n_lit_avail) prefetch_l1(lit + L + 128u * lane);
+        if constexpr (LA) { /* a lane's wait covers its own copies; the warp reads every lane's */
+            cp_async_wait_all();
+            __syncwarp();
+        }
 #if ZXC_STAGE
         const u32 tok_w = ghi ? 4u : 1u, off_w = enc_off ? 1u : 2u;
         const u32 tx0 = (u32)(reinterpret_cast<uintptr_t>(tok) & 15u), ox0 = (u32)(reinterpret_cast<uintptr_t>(offs) & 15u);
@@ -938,19 +1041,29 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
                  * pointer for all three and forms the others from it where they are read */
                 const u8* tk = tok;
                 if constexpr (LEAN) tk = lit + opaque(n_lit_avail);
-                a = tk[i];
+                if constexpr (LA) {
+                    /* the slot holds the aligned words from the one that holds the batch's first token (offset) on */
+                    a = lds8(slot_s + ((u32)reinterpret_cast<uintptr_t>(tk + base) & 3u) + lane);
+                    const u32 ox = (u32)reinterpret_cast<uintptr_t>(tk + n_seq + (enc_off ? base : 2u * base)) & 3u;
+                    const u32 oa = slot_s + LA_OFF + ox + (enc_off ? lane : 2u * lane);
+                    if (enc_off) b = lds8(oa);
+                    else if (ox & 1u) b = lds8(oa) | (lds8(oa + 1u) << 8);
+                    else b = lds16(oa);
+                } else {
+                    a = tk[i];
 #if ZXC_ALIGNED_LD
-                if (LEAN) {
-                    const u32 oi = n_seq + (enc_off ? i : 2u * i);
-                    if (enc_off) b = (u32)tk[oi];
-                    else if ((reinterpret_cast<uintptr_t>(tk) + n_seq) & 1u) b = ld16(tk + oi);
-                    else b = (u32)*reinterpret_cast<const unsigned short*>(tk + oi);
-                } else if (enc_off) b = (u32)offs[i];
-                else if (reinterpret_cast<uintptr_t>(offs) & 1u) b = ld16(offs + 2 * (size_t)i);
-                else b = (u32)reinterpret_cast<const unsigned short*>(offs)[i];
+                    if (LEAN) {
+                        const u32 oi = n_seq + (enc_off ? i : 2u * i);
+                        if (enc_off) b = (u32)tk[oi];
+                        else if ((reinterpret_cast<uintptr_t>(tk) + n_seq) & 1u) b = ld16(tk + oi);
+                        else b = (u32)*reinterpret_cast<const unsigned short*>(tk + oi);
+                    } else if (enc_off) b = (u32)offs[i];
+                    else if (reinterpret_cast<uintptr_t>(offs) & 1u) b = ld16(offs + 2 * (size_t)i);
+                    else b = (u32)reinterpret_cast<const unsigned short*>(offs)[i];
 #else
-                b = enc_off ? (u32)offs[i] : ld16(offs + 2 * (size_t)i);
+                    b = enc_off ? (u32)offs[i] : ld16(offs + 2 * (size_t)i);
 #endif
+                }
             } else {
 #if ZXC_ALIGNED_LD
                 a = (reinterpret_cast<uintptr_t>(tok) & 3u) ? ld32(tok + 4 * (size_t)i) : reinterpret_cast<const u32*>(tok)[i];
@@ -979,11 +1092,19 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             const u32* vt = vals;
             if constexpr (LEAN) vt = esc_table(warp_scratch(P, grid_warp_now()), P.block_cap);
             u32 k = ord_base + __popc(m_ll & lt_mask) + __popc(m_ml & lt_mask);
-            if (e_ll) {
-                ll += k < n_val ? vt[k] : 0u; /* past the last varint the reference reads 0 (:51-88) */
-                k++;
+            if constexpr (LA) { /* the table is read only for ordinals past the staged 32 */
+                if (e_ll) {
+                    ll += la_esc(slot_s, k, ord_base, n_val, P);
+                    k++;
+                }
+                if (e_ml) ml += la_esc(slot_s, k, ord_base, n_val, P);
+            } else {
+                if (e_ll) {
+                    ll += k < n_val ? vt[k] : 0u; /* past the last varint the reference reads 0 (:51-88) */
+                    k++;
+                }
+                if (e_ml) ml += k < n_val ? vt[k] : 0u;
             }
-            if (e_ml) ml += k < n_val ? vt[k] : 0u;
         } else if (ZXC_RARE((m_ll | m_ml) != 0)) {
             const u32 ord_ll = __popc(m_ll & lt_mask) + __popc(m_ml & lt_mask);
             k_esc = __popc(m_ll) + __popc(m_ml);
@@ -1042,6 +1163,10 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             if (!use_vals)
                 for (u32 s = 0; s < q; s++) epos = varint_advance(ext, epos, ext_end); /* rare: re-walk */
             base += 1;
+            if constexpr (LA) {
+                la_issue_words(slot_s, lit + opaque(n_lit_avail), n_seq, enc_off, base, lane);
+                la_issue_esc(slot_s, n_val, ord_base, lane, P);
+            }
             ZXC_TRACE_MARK(TR_GIANT, lane);
             continue;
         }
@@ -1060,6 +1185,15 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             return __shfl_sync(FULL, code, __ffs(m_err) - 1);
         }
         const u32 T = __shfl_sync(FULL, s_tot, m - 1), TL = __shfl_sync(FULL, s_ll, m - 1);
+        if constexpr (LA) {
+            /* the next batch starts at sequence base + m, with the escape ordinal after this batch's: its words are
+             * copied into the slot while this batch copies (the slot's reads are behind the ballot above) */
+            const u32 below = m < 32u ? (1u << m) - 1u : FULL;
+            ord_base += __popc(m_ll & below) + __popc(m_ml & below);
+            base += m;
+            la_issue_words(slot_s, lit + opaque(n_lit_avail), n_seq, enc_off, base, lane);
+            la_issue_esc(slot_s, n_val, ord_base, lane, P);
+        }
 #if ZXC_STAGE && ZXC_STAGE_LIT
         const u32 lx0 = (u32)(reinterpret_cast<uintptr_t>(lit) & 15u);
         const StWindow lw = LitStream::need(stage_s, lit, lx0 + L, lx0 + L + TL, 8u, lane);
@@ -1214,7 +1348,9 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
         __syncwarp();
         ZXC_TRACE_MARK(TR_FLUSH, lane);
 
-        if (m < nvalid) {
+        if constexpr (LA) {
+            /* advanced where the next batch's copies were issued */
+        } else if (m < nvalid) {
             const u32 below = (1u << m) - 1u;
             const u32 q = __popc(m_ll & below) + __popc(m_ml & below);
             ord_base += q;
@@ -1227,6 +1363,7 @@ __device__ int decode_lz_block(const u8* pay, u32 comp, u8* out, u32 cap, const 
             base += 32;
         }
     }
+    if constexpr (LA) cp_async_wait_all(); /* the copies issued for the batch after the last one land before the block ends */
 
     /* trailing literals (zxc_decompress.c:1198-1206) */
     ST_LIT_CLOSE();
@@ -1295,7 +1432,7 @@ __global__ void __launch_bounds__(CTA_THREADS, LEAN ? LEAN_CTAS_PER_SM : CTAS_PE
     const u32 wic = threadIdx.x >> 5;
     const u32 gwarp = blockIdx.x * WARPS_PER_CTA + wic;
     u8* scratch = warp_scratch(P, gwarp);
-    u8* ring = smem + (size_t)wic * WARP_SMEM_BYTES;
+    u8* ring = smem + (size_t)wic * (la_on<HAS_DICT, LEAN>() ? LEAN_WARP_SMEM_BYTES : WARP_SMEM_BYTES); /* the slot behind */
 #if ZXC_STAGE
     st_init(smem_addr(ring) + RING_BYTES, lane);
 #endif

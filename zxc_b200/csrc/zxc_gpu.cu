@@ -346,7 +346,7 @@ extern "C" uint64_t zxc_b200_launch_count(void) { return g_launches; }
 extern "C" int zxc_b200_decode_occupancy(int* lean, int* general) {
     if (zxg_init() != ZXC_OK) return ZXC_B200_ERROR_CUDA;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(lean, zxc_decode_kernel<false, false, false, true>, CTA_THREADS,
-                                                      DECODE_SMEM_BYTES + LEAN_SMEM_PAD) != cudaSuccess ||
+                                                      LEAN_SMEM_BYTES) != cudaSuccess ||
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(general, zxc_decode_kernel<false, true, false, false>, CTA_THREADS,
                                                       DECODE_SMEM_BYTES) != cudaSuccess)
         return ZXC_B200_ERROR_CUDA;
@@ -801,7 +801,7 @@ static int launch_decode_ex(const void* d_src, void* d_dst, const zxc_b200_job_t
             carveout_done = 1;
         }
 #endif
-        const u32 lean_smem = DECODE_SMEM_BYTES + LEAN_SMEM_PAD;
+        const u32 lean_smem = has_dict ? DECODE_SMEM_BYTES + LEAN_SMEM_PAD : LEAN_SMEM_BYTES; /* + look-ahead slots */
         if (has_dict) zxc_decode_kernel<false, false, true, true><<<grid, CTA_THREADS, lean_smem, st>>>(P);
         else zxc_decode_kernel<false, false, false, true><<<grid, CTA_THREADS, lean_smem, st>>>(P);
         __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
