@@ -1242,8 +1242,8 @@ int64_t zxc_write_seek_table(uint8_t* dst, const size_t dst_capacity, const uint
 }
 
 /* ------------------------------------------------------------------------- */
-/* FILE* helpers and push streaming: outside the hot-path scope.             */
-/* Thin host readers where that is all it takes, loud refusal otherwise.     */
+/* FILE* helpers: thin host readers around the buffer API.                  */
+/* (push streaming, zxc_cstream_* / zxc_dstream_*, is in zxc_pstream.c)     */
 /* ------------------------------------------------------------------------- */
 static uint8_t* slurp(FILE* f, size_t* n_out) {
     size_t cap = 1 << 20, n = 0;
@@ -1368,18 +1368,3 @@ int64_t zxc_stream_compress(FILE* f_in, FILE* f_out, const zxc_compress_opts_t* 
     free(in);
     return r;
 }
-
-struct zxc_cstream_s { int unused; };
-struct zxc_dstream_s { int unused; };
-zxc_cstream* zxc_cstream_create(const zxc_compress_opts_t* opts) { (void)opts; return NULL; }
-void zxc_cstream_free(zxc_cstream* cs) { (void)cs; }
-int64_t zxc_cstream_compress(zxc_cstream* cs, zxc_outbuf_t* out, zxc_inbuf_t* in) { (void)cs; (void)out; (void)in; return ZXC_B200_ERROR_UNSUPPORTED; }
-int64_t zxc_cstream_end(zxc_cstream* cs, zxc_outbuf_t* out) { (void)cs; (void)out; return ZXC_B200_ERROR_UNSUPPORTED; }
-size_t zxc_cstream_in_size(const zxc_cstream* cs) { (void)cs; return 0; }
-size_t zxc_cstream_out_size(const zxc_cstream* cs) { (void)cs; return 0; }
-zxc_dstream* zxc_dstream_create(const zxc_decompress_opts_t* opts) { (void)opts; return NULL; }
-void zxc_dstream_free(zxc_dstream* ds) { (void)ds; }
-int64_t zxc_dstream_decompress(zxc_dstream* ds, zxc_outbuf_t* out, zxc_inbuf_t* in) { (void)ds; (void)out; (void)in; return ZXC_B200_ERROR_UNSUPPORTED; }
-int zxc_dstream_finished(const zxc_dstream* ds) { (void)ds; return 0; }
-size_t zxc_dstream_in_size(const zxc_dstream* ds) { (void)ds; return 0; }
-size_t zxc_dstream_out_size(const zxc_dstream* ds) { (void)ds; return 0; }
