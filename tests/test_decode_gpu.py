@@ -320,6 +320,27 @@ def test_frames_with_short_non_final_blocks(prod, ref):
         assert r0s == r1s, (level, r0s, r1s)
 
 
+@pytest.mark.parametrize("body_mib", [1, 40], ids=["in-hbm", "streamed"])
+def test_short_tail_blocks_beyond_the_regular_plan(prod, ref, body_mib):
+    """Full blocks, then two short ones: the regular plan (block i at i*block_size) runs past the capacity at the first
+    short block, so only the full blocks are planned and all of them decode fine.  The general split must still get
+    its turn, whichever route the planned blocks took (40 MiB planned streams through zxg_decode_staged)."""
+    import struct
+    bs = 65536
+    data = zc.silesia_shaped((body_mib << 20) + 2000, seed=23)
+    head, eof, blocks = None, None, []
+    for a, b in ((0, body_mib << 20), (body_mib << 20, (body_mib << 20) + 1000), ((body_mib << 20) + 1000, data.size)):
+        fr = ref.compress(data[a:b], level=3, block_size=bs).tobytes()
+        head, eof = fr[:16], fr[-20:-12]
+        blocks.append(fr[16:-20])
+    frame = np.frombuffer(head + b"".join(blocks) + eof + struct.pack("<QI", data.size, 0), np.uint8)
+    for cap in (data.size, data.size - 1):
+        r0, o0 = ref.decompress(frame, cap)
+        r1, o1 = prod.decompress(frame, cap)
+        assert r1 == r0, (cap, z.ERR.get(r1, r1), r0)
+        assert np.array_equal(o1, o0)
+
+
 def test_deep_skewed_huffman_table_rank_words(prod, ref, orc):
     """ADVICE r1 (high): a Kraft-complete code with lengths 1,2,...,10,11,11 has eleven bitmap levels, each carrying
     every symbol when the runs are all ones -- 11*n/8 bytes of runs, the worst case for the decoder's rank table

@@ -343,7 +343,6 @@ zxc_cctx* zxc_init_static_cctx(void* workspace, const size_t workspace_size, con
 #define ZX_MAX_DEV 16
 typedef struct {
     int device, own_thread;
-    zxg_ctx* g;
     const uint8_t* src;
     zxg_fetch_fn fetch;
     void* fetch_ctx;
@@ -356,17 +355,25 @@ typedef struct {
     uint32_t dict_size;
     const void* dict_huf;
     uint32_t bs;
-    int verify, pinned, rc;
+    int verify, pinned, rc; /* pinned: src and dst are both page-locked */
 } zx_part;
 
+/* One stripe through an overlapped pipeline: zxg_decode_pipelined straight from / into the caller's memory when the
+ * source is memory-backed, both buffers are page-locked and the stripe's blocks are wanted whole; zxg_decode_staged
+ * through the pinned bounce buffers otherwise. */
 static void part_run(zx_part* p, zxg_ctx* g) {
     const uint32_t n = p->n;
-    zxc_b200_job_t* jb = (zxc_b200_job_t*)malloc((size_t)n * sizeof *jb);
-    if (!jb) { p->rc = ZXC_ERROR_MEMORY; return; }
     const uint64_t d0 = p->jobs[0].dst_off, d1 = p->jobs[n - 1].dst_off + p->jobs[n - 1].dst_cap;
-    for (uint32_t i = 0; i < n; i++) {
-        jb[i] = p->jobs[i];
-        jb[i].dst_off -= d0; /* stripe-local decoded coordinates; source offsets stay absolute */
+    const zxc_b200_job_t* jb = p->jobs;
+    zxc_b200_job_t* local = NULL;
+    if (d0 != 0) { /* a later stripe: stripe-local decoded coordinates; source offsets stay absolute */
+        local = (zxc_b200_job_t*)malloc((size_t)n * sizeof *local);
+        if (!local) { p->rc = ZXC_ERROR_MEMORY; return; }
+        for (uint32_t i = 0; i < n; i++) {
+            local[i] = p->jobs[i];
+            local[i].dst_off -= d0;
+        }
+        jb = local;
     }
     const uint64_t src_lo = p->jobs[0].src_off, src_hi = p->jobs[n - 1].src_off + p->jobs[n - 1].src_len;
     const uint64_t lo = p->clip_lo > d0 ? p->clip_lo : d0, hi = p->clip_hi < d1 ? p->clip_hi : d1;
@@ -377,7 +384,7 @@ static void part_run(zx_part* p, zxg_ctx* g) {
     else
         p->rc = zxg_decode_staged(g, p->src, p->fetch, p->fetch_ctx, src_lo, src_hi, out, lo - d0, hi - d0, jb, n, p->st,
                                   p->dict, p->dict_size, p->dict_huf, p->bs, p->verify);
-    free(jb);
+    free(local);
 }
 
 static void* part_main(void* arg) {
@@ -406,34 +413,21 @@ static int multi_devices(uint64_t decoded_bytes) {
     return want < 1 ? 1 : want;
 }
 
-/* jobs (contiguous, dst_off ascending) over D devices; g0 = the caller's context (stripe 0, calling thread) */
-static int decode_multi(int D, zxg_ctx* g0, const uint8_t* src, zxg_fetch_fn fetch, void* fetch_ctx, uint8_t* dst,
-                        uint64_t clip_lo, uint64_t clip_hi, const zxc_b200_job_t* jobs, uint32_t n, int32_t* st,
-                        const void* dict, uint32_t dict_size, const void* dict_huf, uint32_t bs, int verify, int pinned) {
+/* the whole call's jobs (contiguous, dst_off ascending) over D devices; g0 = the caller's context (stripe 0, calling
+ * thread) */
+static int decode_multi(int D, zxg_ctx* g0, const zx_part* whole) {
     zx_part parts[ZX_MAX_DEV];
     pthread_t th[ZX_MAX_DEV];
     const int cur = zxg_current_device(), nd = zxg_device_count();
-    const uint32_t per = (n + (uint32_t)D - 1) / (uint32_t)D;
+    const uint32_t n = whole->n, per = (n + (uint32_t)D - 1) / (uint32_t)D;
     int np = 0;
     for (uint32_t start = 0; start < n && np < ZX_MAX_DEV; start += per, np++) {
         zx_part* p = &parts[np];
-        memset(p, 0, sizeof *p);
+        *p = *whole;
         p->device = (cur + np) % (nd > 0 ? nd : 1);
-        p->src = src;
-        p->fetch = fetch;
-        p->fetch_ctx = fetch_ctx;
-        p->dst = dst;
-        p->clip_lo = clip_lo;
-        p->clip_hi = clip_hi;
-        p->jobs = jobs + start;
+        p->jobs = whole->jobs + start;
         p->n = n - start < per ? n - start : per;
-        p->st = st + start;
-        p->dict = dict;
-        p->dict_size = dict_size;
-        p->dict_huf = dict_huf;
-        p->bs = bs;
-        p->verify = verify;
-        p->pinned = pinned;
+        p->st = whole->st + start;
     }
     for (int k = 1; k < np; k++) parts[k].own_thread = pthread_create(&th[k], NULL, part_main, &parts[k]) == 0;
     part_run(&parts[0], g0);
@@ -447,6 +441,61 @@ static int decode_multi(int D, zxg_ctx* g0, const uint8_t* src, zxg_fetch_fn fet
     for (int k = 0; k < np; k++)
         if (parts[k].rc != ZXC_OK) return parts[k].rc;
     return ZXC_OK;
+}
+
+/* decoded bytes from which a call overlaps H2D, decode and D2H chunk by chunk; below it, one round trip */
+#define STREAM_MIN_BYTES ((uint64_t)32 << 20)
+
+/* The decode of a planned frame or range between host buffers, by one of three routes:
+ *   - may_stream and >= STREAM_MIN_BYTES decoded: decode_multi over several devices when the environment asks for
+ *     it (multi_devices), else one stripe on the caller's context (part_run: pipelined or staged);
+ *   - otherwise in HBM: one H2D of the source span (through a bounce when the source is `fetch`), zxg_decode_jobs, and
+ *     one D2H of [clip_lo, clip_hi) -- only when every job produced its planned size, so a failed small decode leaves
+ *     dst untouched.
+ * Jobs: source offsets absolute (src / fetch coordinates), decoded offsets from 0; decoded bytes [clip_lo, clip_hi)
+ * land at dst.  The per-job statuses in st are the caller's to judge; the return value is ZXC_OK or a failure of the
+ * call itself (memory, CUDA, fetch). */
+static int decode_to_host(zxg_ctx* g, const uint8_t* src, zxg_fetch_fn fetch, void* fetch_ctx, uint8_t* dst,
+                          uint64_t clip_lo, uint64_t clip_hi, const zxc_b200_job_t* jobs, uint32_t n, int32_t* st,
+                          const void* dict, uint32_t dict_size, const void* dict_huf, uint32_t bs, int verify,
+                          int may_stream) {
+    const uint64_t produced = jobs[n - 1].dst_off + jobs[n - 1].dst_cap;
+    if (may_stream && produced >= STREAM_MIN_BYTES) {
+        zx_part whole = {.src = src, .fetch = fetch, .fetch_ctx = fetch_ctx, .dst = dst, .clip_lo = clip_lo,
+                         .clip_hi = clip_hi, .jobs = jobs, .n = n, .st = st, .dict = dict, .dict_size = dict_size,
+                         .dict_huf = dict_huf, .bs = bs, .verify = verify,
+                         .pinned = src && zxg_host_pinned(src) && zxg_host_pinned(dst)};
+        const int D = multi_devices(produced);
+        if (D > 1) return decode_multi(D, g, &whole);
+        part_run(&whole, g);
+        return whole.rc;
+    }
+    const uint64_t src_lo = jobs[0].src_off, src_hi = jobs[n - 1].src_off + jobs[n - 1].src_len;
+    uint8_t* d_in = (uint8_t*)zxg_buffer(g, ZXG_BUF_IN, (size_t)(src_hi - src_lo) + 16);
+    uint8_t* d_out = (uint8_t*)zxg_buffer(g, ZXG_BUF_OUT, (size_t)produced + 16);
+    if (!d_in || !d_out) return ZXC_ERROR_MEMORY;
+    int rc;
+    if (!fetch) {
+        rc = zxg_h2d(g, d_in, src + src_lo, (size_t)(src_hi - src_lo));
+    } else { /* a reader-backed source: pull the compressed span through a host bounce */
+        const size_t chunk = (size_t)16 << 20;
+        uint8_t* bounce = (uint8_t*)malloc(src_hi - src_lo < chunk ? (size_t)(src_hi - src_lo) : chunk);
+        rc = bounce ? ZXC_OK : ZXC_ERROR_MEMORY;
+        for (uint64_t p = src_lo; rc == ZXC_OK && p < src_hi;) {
+            const size_t len = src_hi - p < chunk ? (size_t)(src_hi - p) : chunk;
+            rc = fetch(fetch_ctx, bounce, len, p);
+            if (rc == ZXC_OK) rc = zxg_h2d(g, d_in + (p - src_lo), bounce, len);
+            if (rc == ZXC_OK) rc = zxg_sync(g);
+            p += len;
+        }
+        free(bounce);
+    }
+    if (rc != ZXC_OK) return rc;
+    rc = zxg_decode_jobs(g, d_in - src_lo, d_out, jobs, n, st, dict, dict_size, dict_huf, bs, verify);
+    if (rc != ZXC_OK) return rc;
+    for (uint32_t i = 0; i < n; i++)
+        if (st[i] < 0 || (uint32_t)st[i] != jobs[i].dst_cap) return ZXC_OK;
+    return zxg_d2h(g, dst, d_out + clip_lo, (size_t)(clip_hi - clip_lo));
 }
 
 /* The reference hands every block block_size + ZXC_DECOMPRESS_TAIL_PAD bytes of room (zxc_dispatch.c:902,
@@ -598,44 +647,11 @@ static int64_t decompress_frame(zxg_ctx* g, const uint8_t* src, size_t src_size,
     if (n_fit > 0) {
         status = (int32_t*)malloc(n_fit * sizeof *status);
         if (!status) { ret = ZXC_ERROR_MEMORY; goto out; }
-        const uint64_t src_lo = w.jobs[0].src_off;
-        const uint64_t src_hi = w.jobs[n_fit - 1].src_off + w.jobs[n_fit - 1].src_len;
+        /* in place (source and destination overlap): the whole frame must be on the device before the first decoded
+         * byte comes back, so no streaming */
         const int overlap = (const uint8_t*)src < dst + dst_capacity && dst < (const uint8_t*)src + src_size;
-        if (!overlap && produced >= ((uint64_t)32 << 20) && zxg_host_pinned(src) && zxg_host_pinned(dst)) {
-            /* page-locked caller buffers: overlap H2D, decode and D2H chunk by chunk */
-            const int D = multi_devices(produced);
-            const int prc = D > 1 ? decode_multi(D, g, src, NULL, NULL, dst, 0, produced, w.jobs, (uint32_t)n_fit, status, dict,
-                                                 (uint32_t)dict_size, dict_huf, w.block_size, verify, 1)
-                                  : zxg_decode_pipelined(g, src, src_lo, src_hi, dst, produced, w.jobs, (uint32_t)n_fit, status,
-                                                         dict, (uint32_t)dict_size, dict_huf, w.block_size, verify);
-            if (prc != ZXC_OK) { ret = prc; goto out; }
-            int mm = 0;
-            const int64_t pf = first_failure(status, w.jobs, n_fit, &mm);
-            if (pf < 0 && mm) goto any_split;
-            if (pf < 0) { ret = pf; goto out; }
-            goto decoded;
-        }
-        if (!overlap && produced >= ((uint64_t)32 << 20)) {
-            /* ordinary (pageable) caller memory: the same overlap through pinned bounce buffers and the copy pool */
-            const int D = multi_devices(produced);
-            const int prc = D > 1 ? decode_multi(D, g, src, NULL, NULL, dst, 0, produced, w.jobs, (uint32_t)n_fit, status, dict,
-                                                 (uint32_t)dict_size, dict_huf, w.block_size, verify, 0)
-                                  : zxg_decode_staged(g, src, NULL, NULL, src_lo, src_hi, dst, 0, produced, w.jobs, (uint32_t)n_fit,
-                                                      status, dict, (uint32_t)dict_size, dict_huf, w.block_size, verify);
-            if (prc != ZXC_OK) { ret = prc; goto out; }
-            int mm = 0;
-            const int64_t pf = first_failure(status, w.jobs, n_fit, &mm);
-            if (pf < 0 && mm) goto any_split;
-            if (pf < 0) { ret = pf; goto out; }
-            goto decoded;
-        }
-        uint8_t* d_in = (uint8_t*)zxg_buffer(g, ZXG_BUF_IN, (size_t)(src_hi - src_lo) + 16);
-        uint8_t* d_out = (uint8_t*)zxg_buffer(g, ZXG_BUF_OUT, (size_t)produced + 16);
-        if (!d_in || !d_out) { ret = ZXC_ERROR_MEMORY; goto out; }
-        int rc = zxg_h2d(g, d_in, src + src_lo, (size_t)(src_hi - src_lo));
-        if (rc != ZXC_OK) { ret = rc; goto out; }
-        rc = zxg_decode_jobs(g, d_in - src_lo, d_out, w.jobs, (uint32_t)n_fit, status, dict, (uint32_t)dict_size,
-                             dict_huf, w.block_size, verify);
+        const int rc = decode_to_host(g, src, NULL, NULL, dst, 0, produced, w.jobs, (uint32_t)n_fit, status, dict,
+                                      (uint32_t)dict_size, dict_huf, w.block_size, verify, !overlap);
         if (rc != ZXC_OK) { ret = rc; goto out; }
         /* a short final block is legal when the footer agrees; anything else is decided by the
          * reference's own order: first block error, else capacity, else footer */
@@ -643,8 +659,6 @@ static int64_t decompress_frame(zxg_ctx* g, const uint8_t* src, size_t src_size,
         const int64_t ff = first_failure(status, w.jobs, n_fit, &mismatch);
         if (ff < 0 && mismatch) goto any_split;
         if (ff < 0) { ret = ff; goto out; }
-        rc = zxg_d2h(g, dst, d_out, (size_t)produced);
-        if (rc != ZXC_OK) { ret = rc; goto out; }
     }
     if (n_fit < w.n_jobs && w.end == ZXW_END_EOF && w.footer_size <= dst_capacity) goto any_split; /* short blocks may fit */
     if (0) {
@@ -655,7 +669,7 @@ static int64_t decompress_frame(zxg_ctx* g, const uint8_t* src, size_t src_size,
         produced = p2;
         n_fit = w.n_jobs;
     }
-decoded:
+    /* decoded: capacity, block-stream end, footer size, global hash */
     if (n_fit < w.n_jobs) { ret = ZXC_ERROR_DST_TOO_SMALL; goto out; }
     if (w.end == ZXW_END_BAD_HEADER) { ret = ZXC_ERROR_BAD_HEADER; goto out; }
     if (w.end == ZXW_END_EOF) {
@@ -742,7 +756,7 @@ int64_t zxc_decompress_inplace(void* buffer, const size_t buffer_capacity, const
     const int rc = inplace_probe(comp, comp_size, &d, &m);
     if (rc != ZXC_OK) return rc;
     if (d > buffer_capacity || buffer_capacity - d < m) return ZXC_ERROR_DST_TOO_SMALL;
-    /* source and destination overlap: decompress_frame then takes the staged path, where the whole
+    /* source and destination overlap: decompress_frame then takes the in-HBM route, where the whole
      * frame is on the device before the first decoded byte comes back */
     return decompress_entry(NULL, comp, comp_size, buf, buffer_capacity, opts);
 }
@@ -1129,7 +1143,7 @@ static int64_t seekable_range(zxc_seekable* s, void* dst, size_t dst_capacity, u
     const uint32_t bs = s->tab.block_size;
     const uint32_t b0 = (uint32_t)(offset / bs), b1 = (uint32_t)((offset + len - 1) / bs);
     const uint32_t nb = b1 - b0 + 1;
-    const uint64_t c_lo = s->tab.comp_offsets[b0], c_hi = s->tab.comp_offsets[b1 + 1];
+    const uint64_t c_hi = s->tab.comp_offsets[b1 + 1];
     const uint64_t out_lo = (uint64_t)b0 * bs;
 
     if (nb > s->tab_cap) {
@@ -1148,71 +1162,22 @@ static int64_t seekable_range(zxc_seekable* s, void* dst, size_t dst_capacity, u
     }
     zxc_b200_job_t* jobs = s->jobs_buf;
     int32_t* st = s->st_buf;
-    int64_t ret;
-    uint64_t out_bytes = 0;
-    for (uint32_t i = 0; i < nb; i++) {
-        jobs[i].src_off = s->tab.comp_offsets[b0 + i] - c_lo;
+    for (uint32_t i = 0; i < nb; i++) { /* source offsets in the frame; decoded ones from the first covered block */
+        jobs[i].src_off = s->tab.comp_offsets[b0 + i];
         jobs[i].src_len = s->tab.comp_sizes[b0 + i];
         jobs[i].dst_off = (uint64_t)i * bs;
         jobs[i].dst_cap = expected_block_bytes(s->tab.total, bs, b0 + i);
-        out_bytes = jobs[i].dst_off + jobs[i].dst_cap;
     }
-    int rc;
-    if (s->src && c_hi > s->src_size) { ret = ZXC_ERROR_SRC_TOO_SMALL; goto out; }
-    if (out_bytes >= ((uint64_t)32 << 20)) {
-        /* large range: H2D, decode and D2H overlapped chunk by chunk.  Job source offsets become absolute frame
-         * offsets; decoded coordinates start at the first covered block. */
-        for (uint32_t i = 0; i < nb; i++) jobs[i].src_off += c_lo;
-        const uint64_t clip_lo = offset - out_lo, clip_hi = clip_lo + len;
-        const int aligned = clip_lo == 0 && clip_hi == out_bytes;
-        const int D = multi_devices(out_bytes);
-        if (D > 1)
-            rc = decode_multi(D, g, s->src, s->src ? NULL : seekable_fetch, s, (uint8_t*)dst, clip_lo, clip_hi, jobs, nb, st,
-                              s->dict, (uint32_t)s->dict_size, s->has_dict_huf ? s->dict_huf : NULL, bs, 0,
-                              s->src && zxg_host_pinned(s->src) && zxg_host_pinned(dst));
-        else if (s->src && aligned && zxg_host_pinned(s->src) && zxg_host_pinned(dst))
-            rc = zxg_decode_pipelined(g, s->src, c_lo, c_hi, (uint8_t*)dst, out_bytes, jobs, nb, st, s->dict,
-                                      (uint32_t)s->dict_size, s->has_dict_huf ? s->dict_huf : NULL, bs, 0);
-        else
-            rc = zxg_decode_staged(g, s->src, s->src ? NULL : seekable_fetch, s, c_lo, c_hi, (uint8_t*)dst, clip_lo, clip_hi,
-                                   jobs, nb, st, s->dict, (uint32_t)s->dict_size, s->has_dict_huf ? s->dict_huf : NULL, bs, 0);
-        if (rc != ZXC_OK) { ret = rc; goto out; }
-        int mm = 0;
-        const int64_t pf = first_failure(st, jobs, nb, &mm);
-        ret = pf < 0 ? pf : (int64_t)len;
-        goto out;
-    }
-    uint8_t* d_in = (uint8_t*)zxg_buffer(g, ZXG_BUF_IN, (size_t)(c_hi - c_lo) + 16);
-    uint8_t* d_out = (uint8_t*)zxg_buffer(g, ZXG_BUF_OUT, (size_t)out_bytes + 16);
-    if (!d_in || !d_out) { ret = ZXC_ERROR_MEMORY; goto out; }
-    if (s->src) {
-        rc = zxg_h2d(g, d_in, s->src + c_lo, (size_t)(c_hi - c_lo));
-    } else {
-        /* reader mode, small range: pull the compressed span through a host bounce */
-        const size_t chunk = (size_t)16 << 20;
-        uint8_t* bounce = (uint8_t*)malloc(c_hi - c_lo < chunk ? (size_t)(c_hi - c_lo) : chunk);
-        rc = bounce ? ZXC_OK : ZXC_ERROR_MEMORY;
-        for (uint64_t p = c_lo; rc == ZXC_OK && p < c_hi;) {
-            const size_t n = c_hi - p < chunk ? (size_t)(c_hi - p) : chunk;
-            rc = seekable_fetch(s, bounce, n, p);
-            if (rc == ZXC_OK) rc = zxg_h2d(g, d_in + (p - c_lo), bounce, n);
-            if (rc == ZXC_OK) rc = zxg_sync(g);
-            p += n;
-        }
-        free(bounce);
-    }
-    if (rc != ZXC_OK) { ret = rc; goto out; }
+    if (s->src && c_hi > s->src_size) return ZXC_ERROR_SRC_TOO_SMALL;
+    const uint64_t clip_lo = offset - out_lo;
     /* checksums are never verified on the seekable path (zxc_seekable.c:707, :909) */
-    rc = zxg_decode_jobs(g, d_in, d_out, jobs, nb, st, s->dict, (uint32_t)s->dict_size,
-                         s->has_dict_huf ? s->dict_huf : NULL, bs, 0);
-    if (rc != ZXC_OK) { ret = rc; goto out; }
+    const int rc = decode_to_host(g, s->src, s->src ? NULL : seekable_fetch, s, (uint8_t*)dst, clip_lo, clip_lo + len,
+                                  jobs, nb, st, s->dict, (uint32_t)s->dict_size, s->has_dict_huf ? s->dict_huf : NULL,
+                                  bs, 0, 1);
+    if (rc != ZXC_OK) return rc;
     int mismatch = 0;
     const int64_t ff = first_failure(st, jobs, nb, &mismatch);
-    if (ff < 0) { ret = ff; goto out; }
-    rc = zxg_d2h(g, dst, d_out + (offset - out_lo), len);
-    ret = rc != ZXC_OK ? rc : (int64_t)len;
-out:
-    return ret;
+    return ff < 0 ? ff : (int64_t)len;
 }
 
 int64_t zxc_seekable_decompress_range(zxc_seekable* s, void* dst, const size_t dst_capacity, const uint64_t offset,

@@ -665,10 +665,10 @@ extern "C" size_t zxc_b200_decode_scratch_size(uint32_t block_size) {
 
 /* d_counter: three 64-bit work counters, zeroed here unless `preset` (then the caller has set them already: the
  * device-planned decode starts the claims at its first real job, zxc_dplan.cuh) */
-static int launch_decode_ex(const void* d_src, void* d_dst, const zxc_b200_job_t* d_jobs, u32 n_jobs,
-                            i32* d_status, const void* d_dict, u32 dict_size, const void* d_dict_huf,
-                            void* d_scratch, size_t scratch_size, u32 block_size, int verify,
-                            unsigned long long* d_counter, cudaStream_t st, int preset) {
+static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d_jobs, u32 n_jobs,
+                         i32* d_status, const void* d_dict, u32 dict_size, const void* d_dict_huf,
+                         void* d_scratch, size_t scratch_size, u32 block_size, int verify,
+                         unsigned long long* d_counter, cudaStream_t st, int preset) {
     if (n_jobs == 0) return ZXC_OK;
     DecodeParams P;
     P.src = (const u8*)d_src;
@@ -829,14 +829,6 @@ static int launch_decode_ex(const void* d_src, void* d_dst, const zxc_b200_job_t
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 
-static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d_jobs, u32 n_jobs,
-                         i32* d_status, const void* d_dict, u32 dict_size, const void* d_dict_huf,
-                         void* d_scratch, size_t scratch_size, u32 block_size, int verify,
-                         unsigned long long* d_counter, cudaStream_t st) {
-    return launch_decode_ex(d_src, d_dst, d_jobs, n_jobs, d_status, d_dict, dict_size, d_dict_huf, d_scratch,
-                            scratch_size, block_size, verify, d_counter, st, 0);
-}
-
 /* device scratch one launch over n_jobs blocks needs (without the counter tail) */
 static size_t launch_scratch_bytes(u32 n_jobs, u32 block_size) {
     size_t n = (size_t)grid_for(n_jobs) * WARPS_PER_CTA * scratch_stride_for(block_size);
@@ -859,7 +851,7 @@ extern "C" int zxc_b200_decode_blocks(const void* d_src, void* d_dst, const zxc_
     const size_t usable = (scratch_size - SCRATCH_TAIL) & ~(size_t)7;
     unsigned long long* counter = (unsigned long long*)((u8*)d_scratch + usable);
     return launch_decode(d_src, d_dst, d_jobs, n_jobs, d_status, d_dict, dict_size, d_dict_huf,
-                         d_scratch, usable, block_size, verify_checksums, counter, (cudaStream_t)stream);
+                         d_scratch, usable, block_size, verify_checksums, counter, (cudaStream_t)stream, 0);
 }
 
 /* one 16-byte result slot per device, allocated on first use and kept: no cudaMalloc / cudaFree per call */
@@ -903,6 +895,23 @@ extern "C" int64_t zxc_b200_reduce_status(const int32_t* d_status, const zxc_b20
     return ret;
 }
 
+/* A decode's dictionary into the context's ZXG_BUF_DICT, its 128-byte literal table (when given) right behind it;
+ * both device pointers stay NULL without a dictionary. */
+static int upload_dict(zxg_ctx* c, const void* h_dict, u32 dict_size, const void* h_dict_huf, u8** d_dict,
+                       u8** d_huf) {
+    *d_dict = NULL;
+    *d_huf = NULL;
+    if (!h_dict || !dict_size) return ZXC_OK;
+    *d_dict = (u8*)zxg_buffer(c, ZXG_BUF_DICT, (size_t)dict_size + 128);
+    if (!*d_dict) return ZXC_ERROR_MEMORY;
+    int rc = zxg_h2d(c, *d_dict, h_dict, dict_size);
+    if (rc == ZXC_OK && h_dict_huf) {
+        *d_huf = *d_dict + dict_size;
+        rc = zxg_h2d(c, *d_huf, h_dict_huf, 128);
+    }
+    return rc;
+}
+
 extern "C" int zxg_decode_jobs(zxg_ctx* c, const void* d_src, void* d_dst, const zxc_b200_job_t* h_jobs,
                                uint32_t n_jobs, int32_t* h_status, const void* h_dict, uint32_t dict_size,
                                const void* h_dict_huf, uint32_t block_size, int verify_checksums) {
@@ -912,22 +921,13 @@ extern "C" int zxg_decode_jobs(zxg_ctx* c, const void* d_src, void* d_dst, const
     const size_t scratch_size = launch_scratch_bytes(n_jobs, block_size);
     void* d_scratch = zxg_buffer(c, ZXG_BUF_SCRATCH, scratch_size);
     if (!d_jobs || !d_status || !d_scratch) return ZXC_ERROR_MEMORY;
-    u8* d_dict = NULL;
-    u8* d_huf = NULL;
-    if (h_dict && dict_size) {
-        d_dict = (u8*)zxg_buffer(c, ZXG_BUF_DICT, (size_t)dict_size + 128);
-        if (!d_dict) return ZXC_ERROR_MEMORY;
-        int rc = zxg_h2d(c, d_dict, h_dict, dict_size);
-        if (rc == ZXC_OK && h_dict_huf) {
-            d_huf = d_dict + dict_size;
-            rc = zxg_h2d(c, d_huf, h_dict_huf, 128);
-        }
-        if (rc != ZXC_OK) return rc;
-    }
-    int rc = zxg_h2d(c, d_jobs, h_jobs, (size_t)n_jobs * sizeof(zxc_b200_job_t));
+    u8 *d_dict, *d_huf;
+    int rc = upload_dict(c, h_dict, dict_size, h_dict_huf, &d_dict, &d_huf);
+    if (rc != ZXC_OK) return rc;
+    rc = zxg_h2d(c, d_jobs, h_jobs, (size_t)n_jobs * sizeof(zxc_b200_job_t));
     if (rc != ZXC_OK) return rc;
     rc = launch_decode(d_src, d_dst, d_jobs, n_jobs, d_status, d_dict, dict_size, d_huf, d_scratch,
-                       scratch_size, block_size, verify_checksums, c->counter, c->stream);
+                       scratch_size, block_size, verify_checksums, c->counter, c->stream, 0);
     if (rc != ZXC_OK) return rc;
     if (cudaMemcpyAsync(h_status, d_status, (size_t)n_jobs * sizeof(i32), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess)
         return ZXC_B200_ERROR_CUDA;
@@ -961,18 +961,9 @@ extern "C" int zxg_decode_pipelined(zxg_ctx* c, const uint8_t* h_src, uint64_t s
     const size_t scratch_size = launch_scratch_bytes(n_jobs, block_size);
     void* d_scratch = zxg_buffer(c, ZXG_BUF_SCRATCH, scratch_size);
     if (!d_in || !d_out || !d_jobs || !d_status || !d_scratch) return ZXC_ERROR_MEMORY;
-    u8* d_dict = NULL;
-    u8* d_huf = NULL;
-    if (h_dict && dict_size) {
-        d_dict = (u8*)zxg_buffer(c, ZXG_BUF_DICT, (size_t)dict_size + 128);
-        if (!d_dict) return ZXC_ERROR_MEMORY;
-        int rc = zxg_h2d(c, d_dict, h_dict, dict_size);
-        if (rc == ZXC_OK && h_dict_huf) {
-            d_huf = d_dict + dict_size;
-            rc = zxg_h2d(c, d_huf, h_dict_huf, 128);
-        }
-        if (rc != ZXC_OK) return rc;
-    }
+    u8 *d_dict, *d_huf;
+    int rc = upload_dict(c, h_dict, dict_size, h_dict_huf, &d_dict, &d_huf);
+    if (rc != ZXC_OK) return rc;
     /* the job table goes up chunk by chunk, just ahead of each launch: one copy of the whole table (24 MB for a million
      * 4 KiB records, staged synchronously by the driver when the table is pageable) would sit in front of the first
      * H2D of payload */
@@ -980,7 +971,6 @@ extern "C" int zxg_decode_pipelined(zxg_ctx* c, const uint8_t* h_src, uint64_t s
     for (int i = 0; i < EV_RING; i++)
         if (!c->ev_ring[i] && cudaEventCreateWithFlags(&c->ev_ring[i], cudaEventDisableTiming) != cudaSuccess)
             return ZXC_B200_ERROR_CUDA;
-    int rc = ZXC_OK;
     uint32_t j0 = 0, chunk_no = 0;
     while (j0 < n_jobs && rc == ZXC_OK) {
         /* events are recycled: a wait refers to the record that preceded it, so reuse is safe */
@@ -1000,7 +990,7 @@ extern "C" int zxg_decode_pipelined(zxg_ctx* c, const uint8_t* h_src, uint64_t s
         cudaStreamWaitEvent(c->stream, ev_in, 0);
         if (rc == ZXC_OK)
             rc = launch_decode(d_in - src_lo, d_out, d_jobs + j0, j1 - j0, d_status + j0, d_dict, dict_size, d_huf,
-                               d_scratch, scratch_size, block_size, verify_checksums, c->counter, c->stream);
+                               d_scratch, scratch_size, block_size, verify_checksums, c->counter, c->stream, 0);
         cudaEventRecord(ev_dec, c->stream);
         cudaStreamWaitEvent(c->s_d2h, ev_dec, 0);
         if (rc == ZXC_OK &&
@@ -1057,13 +1047,24 @@ struct staged_chunk {
     uint64_t c0, c1;   /* clipped decoded range delivered to the caller */
 };
 
+/* One past the last job of the chunk that starts at job j0: the whole jobs that fit both an output slot (STAGE_OUT
+ * decoded bytes) and an input slot (STAGE_IN compressed bytes).  j0 itself when job j0 alone does not fit. */
+static uint32_t staged_chunk_end(const zxc_b200_job_t* jobs, uint32_t n_jobs, uint32_t j0) {
+    uint32_t j1 = j0;
+    uint64_t out = 0, in = 0;
+    while (j1 < n_jobs && out + jobs[j1].dst_cap <= STAGE_OUT && in + jobs[j1].src_len <= STAGE_IN) {
+        out += jobs[j1].dst_cap;
+        in += jobs[j1].src_len;
+        j1++;
+    }
+    return j1;
+}
+
 extern "C" int zxg_decode_staged(zxg_ctx* c, const uint8_t* h_src, zxg_fetch_fn fetch, void* fetch_ctx, uint64_t src_lo,
                                  uint64_t src_hi, uint8_t* h_dst, uint64_t clip_lo, uint64_t clip_hi,
                                  const zxc_b200_job_t* h_jobs, uint32_t n_jobs, int32_t* h_status, const void* h_dict,
                                  uint32_t dict_size, const void* h_dict_huf, uint32_t block_size, int verify_checksums) {
     if (n_jobs == 0) return ZXC_OK;
-    struct timespec tw0, tw1, tw2;
-    clock_gettime(CLOCK_MONOTONIC, &tw0);
     int rc = staged_ready(c);
     if (rc != ZXC_OK) return rc;
     const uint64_t produced = h_jobs[n_jobs - 1].dst_off + h_jobs[n_jobs - 1].dst_cap;
@@ -1074,36 +1075,18 @@ extern "C" int zxg_decode_staged(zxg_ctx* c, const uint8_t* h_src, zxg_fetch_fn 
     /* a chunk holds at most STAGE_OUT / (smallest decoded block) jobs; every slot decodes on its own stream with its
      * own scratch region and work counters, so up to STAGE_SLOTS chunk launches are resident together */
     uint32_t chunk_jobs_max = 1;
-    {
-        uint32_t j = 0;
-        while (j < n_jobs) {
-            uint32_t j1 = j;
-            uint64_t ao = 0, ai = 0;
-            while (j1 < n_jobs && ao + h_jobs[j1].dst_cap <= STAGE_OUT && ai + h_jobs[j1].src_len <= STAGE_IN) {
-                ao += h_jobs[j1].dst_cap;
-                ai += h_jobs[j1].src_len;
-                j1++;
-            }
-            if (j1 == j) break;
-            if (j1 - j > chunk_jobs_max) chunk_jobs_max = j1 - j;
-            j = j1;
-        }
+    for (uint32_t j = 0; j < n_jobs;) {
+        const uint32_t j1 = staged_chunk_end(h_jobs, n_jobs, j);
+        if (j1 == j) break;
+        if (j1 - j > chunk_jobs_max) chunk_jobs_max = j1 - j;
+        j = j1;
     }
     const size_t scratch_size = (launch_scratch_bytes(chunk_jobs_max, block_size) + 255) & ~(size_t)255;
     u8* d_scratch = (u8*)zxg_buffer(c, ZXG_BUF_SCRATCH, scratch_size * STAGE_SLOTS);
     if (!d_in || !d_out || !d_jobs || !d_status || !d_scratch) return ZXC_ERROR_MEMORY;
-    u8* d_dict = NULL;
-    u8* d_huf = NULL;
-    if (h_dict && dict_size) {
-        d_dict = (u8*)zxg_buffer(c, ZXG_BUF_DICT, (size_t)dict_size + 128);
-        if (!d_dict) return ZXC_ERROR_MEMORY;
-        rc = zxg_h2d(c, d_dict, h_dict, dict_size);
-        if (rc == ZXC_OK && h_dict_huf) {
-            d_huf = d_dict + dict_size;
-            rc = zxg_h2d(c, d_huf, h_dict_huf, 128);
-        }
-        if (rc != ZXC_OK) return rc;
-    }
+    u8 *d_dict, *d_huf;
+    rc = upload_dict(c, h_dict, dict_size, h_dict_huf, &d_dict, &d_huf);
+    if (rc != ZXC_OK) return rc;
     if (cudaMemcpyAsync(d_jobs, h_jobs, (size_t)n_jobs * sizeof(zxc_b200_job_t), cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
         return ZXC_B200_ERROR_CUDA;
     cudaStreamSynchronize(c->stream); /* h_jobs may be pageable: do not let the caller free it under the copy */
@@ -1112,29 +1095,13 @@ extern "C" int zxg_decode_staged(zxg_ctx* c, const uint8_t* h_src, zxg_fetch_fn 
     uint32_t j0 = 0, issued = 0, drained = 0;
     copy_pool* drain_job = NULL; /* the drain in flight on the second pool ... */
     int drain_slot = -1;         /* ... and the output slot it is reading */
-    const int trace = getenv("ZXC_B200_STAGE_TRACE") != NULL; /* development: where the host thread's time goes */
-    double t_fill = 0, t_drain = 0, t_wait_in = 0, t_wait_out = 0, t_launch = 0;
-    cudaEvent_t tev[STAGE_SLOTS][6]; /* trace only: H2D, decode, D2H brackets of the chunk in each slot */
-    float g_h2d = 0, g_dec = 0, g_d2h = 0, g_lat = 0;
-    if (trace)
-        for (int i = 0; i < STAGE_SLOTS; i++)
-            for (int q = 0; q < 6; q++) cudaEventCreate(&tev[i][q]);
-    struct timespec ts0, ts1;
-#define STG_T0() do { if (trace) clock_gettime(CLOCK_MONOTONIC, &ts0); } while (0)
-#define STG_T1(acc) do { if (trace) { clock_gettime(CLOCK_MONOTONIC, &ts1); acc += (ts1.tv_sec - ts0.tv_sec) + 1e-9 * (ts1.tv_nsec - ts0.tv_nsec); } } while (0)
     while (rc == ZXC_OK && (drained < issued || j0 < n_jobs)) {
         /* one slot is always left to the drain in flight, so filling the next chunk never waits for it */
         if (j0 < n_jobs && issued - drained < STAGE_SLOTS - 1) { /* a slot is free: stage and queue the next chunk */
             const int slot = (int)(issued % STAGE_SLOTS);
             staged_chunk ch;
             ch.j0 = j0;
-            uint32_t j1 = j0;
-            uint64_t acc_out = 0, acc_in = 0;
-            while (j1 < n_jobs && acc_out + h_jobs[j1].dst_cap <= STAGE_OUT && acc_in + h_jobs[j1].src_len <= STAGE_IN) {
-                acc_out += h_jobs[j1].dst_cap;
-                acc_in += h_jobs[j1].src_len;
-                j1++;
-            }
+            const uint32_t j1 = staged_chunk_end(h_jobs, n_jobs, j0);
             if (j1 == j0) { /* a single block larger than a stage: cannot happen with <= 2 MiB blocks */
                 rc = ZXC_ERROR_MEMORY;
                 break;
@@ -1150,85 +1117,51 @@ extern "C" int zxg_decode_staged(zxg_ctx* c, const uint8_t* h_src, zxg_fetch_fn 
                 pool_copy_end(drain_job);
                 drain_job = NULL;
             }
-            STG_T0();
             cudaEventSynchronize(c->st_ev_in[slot]); /* the slot's previous H2D has left the bounce buffer */
-            STG_T1(t_wait_in);
             u8* pin = (u8*)c->st_in[slot].p;
-            STG_T0();
             if (fetch) {
                 rc = fetch(fetch_ctx, pin, (size_t)(ch.s1 - ch.s0), ch.s0);
                 if (rc != ZXC_OK) break;
             } else {
                 pool_memcpy(c->device, pin, h_src + ch.s0, (size_t)(ch.s1 - ch.s0));
             }
-            STG_T1(t_fill);
-            STG_T0();
-            if (trace) cudaEventRecord(tev[slot][0], c->s_h2d);
             if (cudaMemcpyAsync(d_in + (ch.s0 - src_lo), pin, (size_t)(ch.s1 - ch.s0), cudaMemcpyHostToDevice, c->s_h2d) != cudaSuccess) {
                 rc = ZXC_B200_ERROR_CUDA;
                 break;
             }
-            if (trace) cudaEventRecord(tev[slot][1], c->s_h2d);
             cudaEventRecord(c->st_ev_in[slot], c->s_h2d);
             cudaStreamWaitEvent(c->s_dec[slot], c->st_ev_in[slot], 0);
-            if (trace) cudaEventRecord(tev[slot][2], c->s_dec[slot]);
             rc = launch_decode(d_in - src_lo, d_out, d_jobs + j0, j1 - j0, d_status + j0, d_dict, dict_size, d_huf,
                                d_scratch + (size_t)slot * scratch_size, scratch_size, block_size, verify_checksums,
-                               c->counter + 4 * slot, c->s_dec[slot]);
+                               c->counter + 4 * slot, c->s_dec[slot], 0);
             if (rc != ZXC_OK) break;
-            if (trace) cudaEventRecord(tev[slot][3], c->s_dec[slot]);
             cudaEventRecord(c->st_ev_dec[slot], c->s_dec[slot]);
             cudaStreamWaitEvent(c->s_d2h, c->st_ev_dec[slot], 0);
-            if (trace) cudaEventRecord(tev[slot][4], c->s_d2h);
             if (ch.c1 > ch.c0 &&
                 cudaMemcpyAsync(c->st_out[slot].p, d_out + ch.c0, (size_t)(ch.c1 - ch.c0), cudaMemcpyDeviceToHost, c->s_d2h) != cudaSuccess) {
                 rc = ZXC_B200_ERROR_CUDA;
                 break;
             }
-            if (trace) cudaEventRecord(tev[slot][5], c->s_d2h);
             cudaEventRecord(c->st_ev_out[slot], c->s_d2h);
             ring[slot] = ch;
             j0 = j1;
             issued++;
-            STG_T1(t_launch);
             if (j0 < n_jobs && issued - drained < STAGE_SLOTS - 1) continue; /* fill the pipeline before draining */
         }
         /* hand the oldest finished chunk to the caller while the GPU works on the younger ones */
         const int ds = (int)(drained % STAGE_SLOTS);
-        STG_T0();
         if (cudaEventSynchronize(c->st_ev_out[ds]) != cudaSuccess) {
             rc = ZXC_B200_ERROR_CUDA;
             break;
         }
-        STG_T1(t_wait_out);
-        if (trace) {
-            float a = 0, b = 0, d2 = 0, l = 0;
-            cudaEventElapsedTime(&a, tev[ds][0], tev[ds][1]);
-            cudaEventElapsedTime(&b, tev[ds][2], tev[ds][3]);
-            cudaEventElapsedTime(&d2, tev[ds][4], tev[ds][5]);
-            cudaEventElapsedTime(&l, tev[ds][0], tev[ds][5]);
-            g_h2d += a; g_dec += b; g_d2h += d2; g_lat += l;
-        }
         const staged_chunk& dc = ring[ds];
-        STG_T0();
         pool_copy_end(drain_job); /* one drain at a time; the previous one overlapped the fill above */
         drain_job = NULL;
         if (dc.c1 > dc.c0) drain_job = pool_copy_begin(c->device, h_dst + (dc.c0 - clip_lo), c->st_out[ds].p, (size_t)(dc.c1 - dc.c0));
         drain_slot = ds;
-        STG_T1(t_drain);
         drained++;
     }
-    clock_gettime(CLOCK_MONOTONIC, &tw1);
     pool_copy_end(drain_job);
-    clock_gettime(CLOCK_MONOTONIC, &tw2);
-    if (trace)
-        fprintf(stderr, "staged decode: %u chunks; host seconds: fill %.4f, enqueue %.4f, drain %.4f, waiting for H2D slot %.4f, "
-                        "waiting for D2H %.4f; loop %.4f, last drain %.4f; device ms summed over chunks: H2D %.1f decode %.1f D2H %.1f, "
-                        "H2D start to D2H end %.1f\n", issued, t_fill, t_launch, t_drain, t_wait_in, t_wait_out,
-                (tw1.tv_sec - tw0.tv_sec) + 1e-9 * (tw1.tv_nsec - tw0.tv_nsec), (tw2.tv_sec - tw1.tv_sec) + 1e-9 * (tw2.tv_nsec - tw1.tv_nsec), g_h2d, g_dec, g_d2h, g_lat);
-    if (trace)
-        for (int i = 0; i < STAGE_SLOTS; i++)
-            for (int q = 0; q < 6; q++) cudaEventDestroy(tev[i][q]);
     cudaError_t e0 = cudaSuccess;
     for (int i = 0; i < STAGE_SLOTS; i++) {
         const cudaError_t e = cudaStreamSynchronize(c->s_dec[i]);
@@ -1634,8 +1567,8 @@ extern "C" int zxg_decompress_device(const void* d_src, uint64_t src_size, void*
     for (u32 b = ZXC_BLOCK_SIZE_MIN; b <= bs; b <<= 1) {
         const u32 lg = (u32)__builtin_ctz(b) - ZXC_BLOCK_SIZE_MIN_LOG2;
         for (int v = 0; v <= (checksum_enabled ? 1 : 0); v++) {
-            const int rc = launch_decode_ex(d_src, d_dst, A.jobs, L.J, A.status, d_dict, dict_size, d_huf, dec,
-                                            L.dec_bytes, b, v, S->ctr[lg * 2 + v], st, 1);
+            const int rc = launch_decode(d_src, d_dst, A.jobs, L.J, A.status, d_dict, dict_size, d_huf, dec,
+                                         L.dec_bytes, b, v, S->ctr[lg * 2 + v], st, 1);
             if (rc != ZXC_OK) return rc;
         }
     }
