@@ -163,6 +163,79 @@ ZXC_EXPORT int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, 
                                           const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
                                           int64_t* d_result, void* stream);
 
+/* ---- random access into a seekable frame in HBM: the device twin of zxc_seekable_open +
+ *      zxc_seekable_decompress_range, for many ranges per call ---- */
+typedef struct zxc_b200_seekable_device_s zxc_b200_seekable_device;
+/* decoded bytes [offset, offset + len) go to d_dst + dst_off */
+typedef struct {
+    uint64_t offset;
+    uint64_t len;
+    uint64_t dst_off;
+} zxc_b200_range_t;
+
+/* Opens the seekable frame d_src[0 .. src_size) (device memory, borrowed like zxc_seekable_open's src: it must stay
+ * valid and unchanged while the handle is used).  Synchronous: the SEK table is parsed on the host from a few copies
+ * made on `stream`, and its block offsets (num_blocks + 1 x 8 bytes) are uploaded once to memory the handle owns, on
+ * the current device, to which the handle is bound.  Returns NULL exactly where zxc_seekable_open returns NULL for the
+ * same bytes, and when there is no device or an allocation fails. */
+ZXC_EXPORT zxc_b200_seekable_device* zxc_b200_seekable_device_open(const void* d_src, uint64_t src_size, void* stream);
+
+/* zxc_seekable_set_dict for the device handle: host pointers, the same verdicts in the same order (NULL_INPUT,
+ * DICT_TOO_LARGE, DICT_MISMATCH; a rejected call leaves the handle unchanged), then ZXC_ERROR_MEMORY when the device
+ * copy cannot be allocated (the previous dictionary is dropped then, as zxc_seekable_set_dict does).  The dictionary and
+ * its 128-byte table are copied to the device here, once; the call waits for the handle's device before it frees a
+ * previous copy. */
+ZXC_EXPORT int zxc_b200_seekable_device_set_dict(zxc_b200_seekable_device* h, const void* dict, size_t dict_size,
+                                                 const void* dict_huf);
+ZXC_EXPORT uint32_t zxc_b200_seekable_device_num_blocks(const zxc_b200_seekable_device* h);
+ZXC_EXPORT uint64_t zxc_b200_seekable_device_decompressed_size(const zxc_b200_seekable_device* h);
+ZXC_EXPORT uint32_t zxc_b200_seekable_device_block_size(const zxc_b200_seekable_device* h);
+
+/* Device scratch for one zxc_b200_seekable_device_decompress_ranges call of at most max_ranges ranges whose lengths
+ * add up to at most max_bytes (0: NULL handle, no device, or a size that cannot be planned).  Every range decodes
+ * whole blocks: a block it covers whole decodes in place in d_dst, a block it covers in part (at most its first and
+ * last) into a slot of block_size bytes in the scratch.  The slots dominate for many small ranges: 2 x max_ranges x
+ * block_size, so 1 024 ranges at 64 KiB blocks take 128 MiB and 16 384 ranges 2 GiB.  On top come the job table
+ * (28 bytes per block of max_bytes), about 90 bytes per range, and the decode kernels' per-warp scratch: one region
+ * of about 2.7 x block_size (180 KiB at 64 KiB blocks, 5.3 MiB at 2 MiB) per warp of the larger of the two decode
+ * launches, which run one warp per job up to the resident grid.  That is W = max(ceil(max_bytes / block_size),
+ * 2 x max_ranges) warps rounded up to 4, and at most the grid's 4 224 warps on an H100 (132 SMs): a single short range
+ * at 2 MiB blocks takes 22 MB, while 2 112 or more ranges, or 4 224 or more blocks of max_bytes, take the full grid:
+ * 768 MB at 64 KiB blocks and 23 GB at 2 MiB. */
+ZXC_EXPORT size_t zxc_b200_seekable_device_scratch_size(const zxc_b200_seekable_device* h, uint32_t max_ranges,
+                                                        uint64_t max_bytes);
+
+/* Decodes n_ranges ranges of the handle's frame on `stream`, asynchronously, with no host synchronisation and no
+ * allocation: the call may be captured in a CUDA graph, with or without a dictionary.  A captured call keeps what it
+ * read from the handle when it was captured -- the dictionary's device copy, whether one was set, the block table --
+ * and the job-table size it took from the scratch: zxc_b200_seekable_device_set_dict or _free invalidates every graph
+ * captured on the handle before (a replay would read freed memory, or give the old DICT_REQUIRED), so capture again
+ * after either.  The contents of d_ranges, d_dst and d_results may change between replays.  d_ranges (n_ranges entries)
+ * and d_results (one int64 per range) are device memory; the call runs on the handle's device and restores the
+ * current device.  Calls on different streams with separate scratch may run at the same time.
+ * Returns ZXC_OK once enqueued, or what the host decides: ZXC_ERROR_NULL_INPUT for a NULL handle, or for a NULL
+ * d_ranges, d_results or d_scratch when n_ranges > 0; ZXC_B200_ERROR_NO_DEVICE; ZXC_ERROR_MEMORY when scratch_size is
+ * below zxc_b200_seekable_device_scratch_size(h, n_ranges, 0).  n_ranges == 0 returns ZXC_OK and launches nothing.
+ * d_results[i] is what zxc_seekable_decompress_range(s, d_dst + dst_off, cap, offset, len) of this library returns on
+ * a handle opened on the same bytes with the same dictionary, where cap = dst_capacity - dst_off (0 when dst_off >
+ * dst_capacity), in its order: 0 for len == 0, NULL_INPUT for a NULL d_dst, DST_TOO_SMALL, SRC_TOO_SMALL (also when
+ * offset + len wraps), DICT_REQUIRED, then the first covered block in block order that failed (its own code, or
+ * CORRUPT_DATA for another size than expected), else len.  Checksums are not verified, as on the host's seekable path.
+ * One more verdict of this call comes between DICT_REQUIRED and the blocks: ranges take job-table entries in index
+ * order, and from the first range whose blocks no longer fit the table the scratch holds, every range that passed
+ * the checks gets ZXC_ERROR_MEMORY and decodes nothing; that happens only when the ranges' lengths add up to more
+ * than the max_bytes the scratch was sized for.
+ * Nothing outside the union of d_dst[dst_off, dst_off + len) over the ranges, the scratch and d_results is written; a
+ * range with a negative result may leave its span partly written, and overlapping spans get unspecified bytes.  Reads
+ * of d_src stay inside the bounds documented for zxc_b200_decompress_device.  Kernel launches per call
+ * (zxc_b200_launch_count): 8 (plan: 3; the decode kernels' lean and general instance on the blocks decoded in place,
+ * then on the slots: 4; finish: 1), whatever the ranges. */
+ZXC_EXPORT int zxc_b200_seekable_device_decompress_ranges(zxc_b200_seekable_device* h,
+                                                          const zxc_b200_range_t* d_ranges, uint32_t n_ranges,
+                                                          void* d_dst, uint64_t dst_capacity, void* d_scratch,
+                                                          size_t scratch_size, int64_t* d_results, void* stream);
+ZXC_EXPORT void zxc_b200_seekable_device_free(zxc_b200_seekable_device* h);
+
 /* Kernels launched by this library since load (for bench.py's gpu_launches). */
 ZXC_EXPORT uint64_t zxc_b200_launch_count(void);
 

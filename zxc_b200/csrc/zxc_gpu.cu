@@ -30,6 +30,7 @@
 #include "zxc_encode.cuh"
 #include "zxc_assemble.cuh"
 #include "zxc_dplan.cuh"
+#include "zxc_dseek.cuh"
 #include "zxc_train.cuh"
 
 /* ========================================================================= */
@@ -1594,6 +1595,157 @@ extern "C" int zxg_decompress_device(const void* d_src, uint64_t src_size, void*
     else launch_dsplit<false>(D, 1, dec_grid, st);
     zxc_dsplit_final<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
     __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* random access into a seekable frame in HBM                                */
+/* (zxc_b200_seekable_device_*: zxc_dseek.c drives these, kernels in         */
+/* zxc_dseek.cuh)                                                            */
+/* ------------------------------------------------------------------------- */
+extern "C" int zxg_d2h_sync(void* h_dst, const void* d_src, size_t bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (cudaMemcpyAsync(h_dst, d_src, bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess) {
+        cudaGetLastError();
+        return ZXC_B200_ERROR_CUDA;
+    }
+    return ZXC_OK;
+}
+
+extern "C" int zxg_h2d_sync(void* d_dst, const void* h_src, size_t bytes, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    if (cudaMemcpyAsync(d_dst, h_src, bytes, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess) {
+        cudaGetLastError();
+        return ZXC_B200_ERROR_CUDA;
+    }
+    return ZXC_OK;
+}
+
+extern "C" void* zxg_dev_alloc(size_t bytes) {
+    void* d = NULL;
+    if (cudaMalloc(&d, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return NULL;
+    }
+    return d;
+}
+
+extern "C" void zxg_dev_free(void* d) {
+    if (!d) return;
+    cudaDeviceSynchronize(); /* range calls still in flight on any stream may read it */
+    cudaFree(d);
+}
+
+/* Scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned):
+ *   DSeekState | per-range records (n) | tile sums | slot table (2n jobs, 2n status) | direct table (J jobs, J status) |
+ *   slots (2n x round_up(block_size, 16)) | decode scratch (per-warp regions, deferred list)
+ * The decode scratch holds the per-warp regions of the larger of the two decode launches, grid_for(max(J, 2n)) warps,
+ * so a call with few ranges and few blocks needs no more than its launches use.  total grows with J, and the call
+ * takes the largest J whose layout fits the scratch it is given. */
+struct DSeekLayout {
+    size_t recs, tiles, sjobs, sstatus, djobs, dstatus, slots, dec, dec_bytes, total;
+    u32 J, stride;
+};
+#define DS_J_MAX 0x7FFFFFFFu
+#define DS_RANGES_MAX (1u << 30) /* the slot table's 2n entries stay below 2^31 */
+
+static void ds_layout(u32 bs, u32 n, u32 J, DSeekLayout* L) {
+    size_t o = DS_STATE_BYTES;
+    L->recs = o;
+    o += r256((size_t)n * sizeof(DSeekRec));
+    L->tiles = o;
+    o += r256(((size_t)n + ASM_TILE - 1) / ASM_TILE * 16);
+    L->sjobs = o;
+    o += r256((size_t)2 * n * sizeof(zxc_b200_job_t));
+    L->sstatus = o;
+    o += r256((size_t)2 * n * 4);
+    L->djobs = o;
+    o += r256((size_t)J * sizeof(zxc_b200_job_t));
+    L->dstatus = o;
+    o += r256((size_t)J * 4);
+    L->stride = (bs + 15u) & ~15u;
+    L->slots = o;
+    o += r256((size_t)2 * n * L->stride);
+    L->dec = o;
+    L->dec_bytes = launch_scratch_bytes(J > 2 * n ? J : 2 * n, bs);
+    L->total = o + L->dec_bytes + 256; /* base alignment slack */
+    L->J = J;
+}
+
+extern "C" size_t zxg_dseek_scratch_bytes(uint32_t block_size, uint32_t n_ranges, uint64_t J) {
+    if (zxg_init() != ZXC_OK || J > DS_J_MAX || n_ranges > DS_RANGES_MAX) return 0;
+    DSeekLayout L;
+    ds_layout(block_size, n_ranges, J < 1 ? 1u : (u32)J, &L);
+    return L.total;
+}
+
+extern "C" int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_ranges, uint32_t n_ranges, void* d_dst,
+                                uint64_t dst_capacity, void* d_scratch, size_t scratch_size, int64_t* d_results,
+                                void* stream) {
+    const u32 bs = h->block_size, n = n_ranges;
+    if (n > DS_RANGES_MAX) return ZXC_ERROR_MEMORY;
+    DSeekLayout L;
+    ds_layout(bs, n, 1, &L);
+    if (L.total > scratch_size) return ZXC_ERROR_MEMORY;
+    /* the largest direct table whose layout fits: L.total grows with J */
+    u32 lo = 1, hi = DS_J_MAX;
+    while (lo < hi) {
+        const u32 mid = lo + (hi - lo + 1) / 2;
+        ds_layout(bs, n, mid, &L);
+        if (L.total <= scratch_size) lo = mid;
+        else hi = mid - 1;
+    }
+    ds_layout(bs, n, lo, &L);
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    DSeekState* S = (DSeekState*)base;
+    const bool has_dict = h->d_dict && h->dict_size;
+    DSeekArgs A;
+    A.offs = (const unsigned long long*)h->d_offs;
+    A.ranges = d_ranges;
+    A.dst = (u8*)d_dst;
+    A.slots = base + L.slots;
+    A.results = (long long*)d_results;
+    A.st = S;
+    A.recs = (DSeekRec*)(base + L.recs);
+    A.tiles = (unsigned long long*)(base + L.tiles);
+    A.djobs = (zxc_b200_job_t*)(base + L.djobs);
+    A.dstatus = (i32*)(base + L.dstatus);
+    A.sjobs = (zxc_b200_job_t*)(base + L.sjobs);
+    A.sstatus = (i32*)(base + L.sstatus);
+    A.total = h->total;
+    A.dst_capacity = dst_capacity;
+    A.n = n;
+    A.J = L.J;
+    A.block_size = bs;
+    A.slot_stride = L.stride;
+    A.need_dict = h->dict_id != 0 && !has_dict;
+    const u32 n_tiles = (n + ASM_TILE - 1) / ASM_TILE;
+    /* a warp per range, and enough threads to zero the status words in front of both tables quickly */
+    const u64 by_ranges = ((u64)n * 32 + DS_THREADS - 1) / DS_THREADS;
+    u64 by_zero = ((u64)L.J + 2ull * n + DS_THREADS * 16 - 1) / (DS_THREADS * 16);
+    if (by_zero > 4096) by_zero = 4096;
+    const u32 emit_grid = (u32)(by_ranges > by_zero ? by_ranges : by_zero);
+    zxc_dseek_tiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dseek_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_dseek_emit<<<emit_grid, DS_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 3, __ATOMIC_RELAXED);
+    if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    /* the blocks covered whole, in place; then the partly covered ones into their slots.  Stream order lets the two
+     * runs share the per-warp scratch and the deferred list; each has its own counters. */
+    u8* dec = base + L.dec;
+    const void* dict = has_dict ? h->d_dict : NULL;
+    const void* huf = has_dict ? h->d_dict_huf : NULL;
+    int rc = launch_decode(h->d_src, d_dst, A.djobs, L.J, A.dstatus, dict, h->dict_size, huf, dec, L.dec_bytes, bs, 0,
+                           S->ctr[0], st, 1);
+    if (rc != ZXC_OK) return rc;
+    rc = launch_decode(h->d_src, A.slots, A.sjobs, 2 * n, A.sstatus, dict, h->dict_size, huf, dec, L.dec_bytes, bs, 0,
+                       S->ctr[1], st, 1);
+    if (rc != ZXC_OK) return rc;
+    zxc_dseek_finish<<<n, DS_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 

@@ -82,6 +82,27 @@ int zxg_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uin
                           int huf_verdict, int checksum_enabled, void* d_scratch, size_t scratch_size,
                           int64_t* d_result, void* stream);
 
+/* Device-resident seekable frames (zxc_dseek.c; kernels in zxc_dseek.cuh).  What a range call needs of its handle. */
+typedef struct {
+    const void* d_src;
+    const uint64_t* d_offs; /* comp_offsets: num_blocks + 1 entries */
+    uint64_t total;
+    uint32_t block_size, num_blocks, dict_id;
+    const void* d_dict; /* NULL without a dictionary; its 128-byte table right behind it when d_dict_huf is set */
+    uint32_t dict_size;
+    const void* d_dict_huf;
+} zxg_dseek_t;
+/* synchronous copies on `stream`, and device memory for a handle (zxg_dev_free waits for the current device first) */
+int zxg_d2h_sync(void* h_dst, const void* d_src, size_t bytes, void* stream);
+int zxg_h2d_sync(void* d_dst, const void* h_src, size_t bytes, void* stream);
+void* zxg_dev_alloc(size_t bytes);
+void zxg_dev_free(void* d);
+/* scratch for n_ranges ranges with a direct job table of J entries (0 when that cannot be planned) */
+size_t zxg_dseek_scratch_bytes(uint32_t block_size, uint32_t n_ranges, uint64_t J);
+/* enqueues the plan, the two decodes and the finish; ZXC_ERROR_MEMORY for a scratch below one job-table entry */
+int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_ranges, uint32_t n_ranges, void* d_dst,
+                     uint64_t dst_capacity, void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);
+
 /* Device selection for the calling thread (multi-device fork-join in zxc_api.c): current device, device count,
  * cudaSetDevice.  zxg_acquire() hands out a context of the calling thread's current device. */
 int zxg_current_device(void);

@@ -3,7 +3,8 @@
 ``compress`` runs zxc_b200_compress_device: the frame is encoded and assembled in HBM on a CUDA stream, with no copy
 through the host.  ``decompress`` decodes such a frame with zxc_b200_decode_blocks from the decode plan the
 compress call emitted.  ``decompress_frame`` decodes any frame held in a uint8 CUDA tensor with
-zxc_b200_decompress_device, which plans, decodes and checks it on the device.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
+zxc_b200_decompress_device, which plans, decodes and checks it on the device.  ``SeekableFrame`` decodes byte ranges of
+a seekable frame in HBM with zxc_b200_seekable_device_decompress_ranges.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
 """
 import ctypes as C
 from dataclasses import dataclass
@@ -217,3 +218,155 @@ def decompress_frame(frame, *, capacity=None, dict=None, dict_huf=None, checksum
     if r < 0:
         raise ZxcError(r, "zxc_b200_decompress_device")
     return out[:r]
+
+
+lib.zxc_b200_seekable_device_open.restype = C.c_void_p
+lib.zxc_b200_seekable_device_open.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
+lib.zxc_b200_seekable_device_set_dict.restype = C.c_int
+lib.zxc_b200_seekable_device_set_dict.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+lib.zxc_b200_seekable_device_num_blocks.restype = C.c_uint32
+lib.zxc_b200_seekable_device_num_blocks.argtypes = [C.c_void_p]
+lib.zxc_b200_seekable_device_decompressed_size.restype = C.c_uint64
+lib.zxc_b200_seekable_device_decompressed_size.argtypes = [C.c_void_p]
+lib.zxc_b200_seekable_device_block_size.restype = C.c_uint32
+lib.zxc_b200_seekable_device_block_size.argtypes = [C.c_void_p]
+lib.zxc_b200_seekable_device_scratch_size.restype = C.c_size_t
+lib.zxc_b200_seekable_device_scratch_size.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64]
+lib.zxc_b200_seekable_device_decompress_ranges.restype = C.c_int
+lib.zxc_b200_seekable_device_decompress_ranges.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64,
+                                                           C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+lib.zxc_b200_seekable_device_free.restype = None
+lib.zxc_b200_seekable_device_free.argtypes = [C.c_void_p]
+
+
+def _check_out(out, device):
+    """An output the range call may write out.numel() bytes into from out.data_ptr(): a contiguous uint8 tensor on
+    the frame's CUDA device.  ValueError otherwise, before anything is enqueued."""
+    if out.dtype != torch.uint8:
+        raise ValueError(f"out must be a uint8 tensor, not {out.dtype}")
+    if not out.is_contiguous():
+        raise ValueError("out must be contiguous")
+    if out.device != device:
+        raise ValueError(f"out must be on the frame's device {device}, not {out.device}")
+
+
+class SeekableFrame:
+    """Random access into a seekable ZXC frame held in a contiguous uint8 CUDA tensor.
+
+    Opens the frame with zxc_b200_seekable_device_open (the SEK table is parsed once; its block offsets stay on the
+    device) and decodes byte ranges of the decompressed content with zxc_b200_seekable_device_decompress_ranges.  The
+    frame tensor is kept alive and must not change while the object is open.  dict / dict_huf are host bytes, set
+    with zxc_b200_seekable_device_set_dict.  Raises ValueError when the frame is not seekable (where
+    zxc_seekable_open returns NULL) and ZxcError for a rejected dictionary."""
+
+    def __init__(self, frame, dict=None, dict_huf=None):
+        self._h = None  # before any check: __del__ runs on a half-made object too
+        if not frame.is_cuda or frame.dtype != torch.uint8 or not frame.is_contiguous():
+            raise ValueError("frame must be a contiguous uint8 CUDA tensor")
+        self.frame = frame.reshape(-1)
+        with torch.cuda.device(self.frame.device):
+            h = lib.zxc_b200_seekable_device_open(self.frame.data_ptr(), self.frame.numel(),
+                                                  torch.cuda.current_stream().cuda_stream)
+        if not h:
+            raise ValueError("not a seekable ZXC frame (or no device)")
+        self._h = h
+        if dict is not None:
+            d = bytes(dict)
+            hf = bytes(dict_huf) if dict_huf is not None else None
+            rc = lib.zxc_b200_seekable_device_set_dict(self._h, d, len(d), hf)
+            if rc != 0:
+                self.close()
+                raise ZxcError(rc, "zxc_b200_seekable_device_set_dict")
+
+    @property
+    def decompressed_size(self):
+        return int(lib.zxc_b200_seekable_device_decompressed_size(self._handle()))
+
+    @property
+    def block_size(self):
+        return int(lib.zxc_b200_seekable_device_block_size(self._handle()))
+
+    @property
+    def n_blocks(self):
+        return int(lib.zxc_b200_seekable_device_num_blocks(self._handle()))
+
+    def _handle(self):
+        if self._h is None:
+            raise ValueError("SeekableFrame is closed")
+        return self._h
+
+    def close(self):
+        if self._h is not None:
+            lib.zxc_b200_seekable_device_free(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        self.close()
+
+    def gather(self, offsets, lengths, out=None, stream=None):
+        """Decode the ranges [offsets[i], offsets[i] + lengths[i]) back to back into one uint8 tensor.
+
+        offsets and lengths are int64 CUDA tensors of one length; range i lands at the sum of the lengths before it
+        (an exclusive cumsum computed on the device).  Returns (out, results) with no synchronisation when `out` is
+        given (its size bounds the scratch); without it, the total length is read back once to allocate out.  `out`
+        must be a contiguous uint8 tensor on the frame's device (ValueError otherwise).  The work runs on `stream`
+        (default: the current stream), which first waits for the current stream; the returned tensors are written on
+        `stream`, so a caller reading them on another stream orders it after `stream` first.
+        results[i] (int64, on the device) is the range's byte count or a negative zxc_error_t code, exactly what
+        zxc_seekable_decompress_range returns for it; the bytes of a failed range are unspecified."""
+        h = self._handle()
+        dev = self.frame.device
+        if out is not None:
+            _check_out(out, dev)
+        offsets = offsets.reshape(-1).to(dev, torch.int64)
+        lengths = lengths.reshape(-1).to(dev, torch.int64)
+        if offsets.numel() != lengths.numel():
+            raise ValueError("offsets and lengths differ in length")
+        n = offsets.numel()
+        with torch.cuda.device(dev):
+            current = torch.cuda.current_stream(dev)
+            stream = stream or current
+            if stream != current:
+                # the inputs were made (or written) on the current stream; the caller may drop them on return
+                stream.wait_stream(current)
+                for t in (offsets, lengths) + ((out,) if out is not None else ()):
+                    t.record_stream(stream)
+            with torch.cuda.stream(stream):
+                dst_off = torch.cumsum(lengths, 0) - lengths
+                if out is None:
+                    out = torch.empty(int(lengths.sum().item()) if n else 0, dtype=torch.uint8, device=dev)
+                results = torch.empty(n, dtype=torch.int64, device=dev)
+                if n == 0:
+                    return out, results
+                ranges = torch.stack([offsets, lengths, dst_off], 1).contiguous()
+                scratch_size = int(lib.zxc_b200_seekable_device_scratch_size(h, n, out.numel()))
+                if scratch_size == 0:
+                    raise ValueError("zxc_b200_seekable_device_scratch_size: too many ranges or bytes")
+                scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
+                rc = lib.zxc_b200_seekable_device_decompress_ranges(
+                    h, ranges.data_ptr(), n, out.data_ptr() if out.numel() else None, out.numel(), scratch.data_ptr(),
+                    scratch_size, results.data_ptr(), stream.cuda_stream)
+                if rc != 0:
+                    raise ZxcError(rc, "zxc_b200_seekable_device_decompress_ranges")
+        return out, results
+
+    def read(self, offset, length, stream=None):
+        """Decode bytes [offset, offset + length) into a new uint8 tensor; synchronises and raises ZxcError with the
+        exact code of zxc_seekable_decompress_range on failure."""
+        dev = self.frame.device
+        o = torch.tensor([int(offset)], dtype=torch.int64, device=dev)
+        n = torch.tensor([int(length)], dtype=torch.int64, device=dev)
+        out = torch.empty(int(length), dtype=torch.uint8, device=dev)
+        stream = stream or torch.cuda.current_stream(dev)
+        out, res = self.gather(o, n, out=out, stream=stream)
+        stream.synchronize()
+        r = int(res.item())
+        if r < 0:
+            raise ZxcError(r, "zxc_b200_seekable_device_decompress_ranges")
+        return out
