@@ -28,8 +28,7 @@
 extern "C" {
 #endif
 
-/* One independent block = one unit of work (a CTA of the block-cooperative kernel, or a warp of
- * the general kernel).  Replaces the reference's
+/* One independent block = one unit of work (a warp of the decode kernel).  Replaces the reference's
  * zxc_seek_mt_job_t (src/lib/zxc_seekable.c:802-815). */
 typedef struct {
     uint64_t src_off; /* byte offset of the 8-byte block header inside the source buffer */

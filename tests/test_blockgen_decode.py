@@ -729,9 +729,9 @@ print("alt ok", n)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("env", [{"ZXC_B200_UNITS": "1"}, {"ZXC_B200_DECODE_V2": "1"}], ids=["unit-walk-forced", "block-cooperative"])
+@pytest.mark.parametrize("env", [{"ZXC_B200_UNITS": "1"}], ids=["unit-walk-forced"])
 def test_gpu_alternative_bodies_on_the_catalogue(env):
-    """the output-centric body and the block-cooperative kernel, selected per process by environment variables"""
+    """the output-centric body, selected per process by an environment variable"""
     e = dict(os.environ)
     e.update(env)
     here = os.path.dirname(os.path.abspath(__file__))

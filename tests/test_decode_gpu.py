@@ -399,10 +399,10 @@ print("alt-body ok", n_ok)
 """
 
 
-@pytest.mark.parametrize("env", [{"ZXC_B200_UNITS": "1"}, {"ZXC_B200_DECODE_V2": "1"}], ids=["unit-walk-forced", "block-cooperative"])
+@pytest.mark.parametrize("env", [{"ZXC_B200_UNITS": "1"}], ids=["unit-walk-forced"])
 def test_alternative_decode_bodies_stay_bit_exact(env):
-    """The output-centric body outside its default domain and the block-cooperative kernel (off by default, DESIGN.md
-    3c) are selected by environment variables read once per process, so they run in a child process."""
+    """The output-centric body outside its default domain is selected by an environment variable read once per
+    process, so it runs in a child process."""
     import subprocess
     import sys
     e = dict(os.environ)

@@ -12,7 +12,7 @@ block_size / 5 + 16, empty token sections, lit_comp / tok_comp bounds).
 Each case must agree with the generator's own tree-walking decoder, the oracle's block decoder and the unmodified
 reference library, which decides every verdict; then with the kernel on the CPU warp emulator (general instance under
 three lane schedules, the two-launch lean route, guard pages) and on the GPU (zxc_b200_decode_blocks, zxc_decompress,
-zxc_decompress_block, the unit-walk and block-cooperative bodies).  On the emulator each case also asserts that the
+zxc_decompress_block, the unit-walk body).  On the emulator each case also asserts that the
 decoder path it targets was taken (ZXC_STAT counters of tests/simt)."""
 import ctypes as C
 import os
@@ -794,7 +794,7 @@ print("alt ok", n)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("env", [{"ZXC_B200_UNITS": "1"}, {"ZXC_B200_DECODE_V2": "1"}], ids=["unit-walk-forced", "block-cooperative"])
+@pytest.mark.parametrize("env", [{"ZXC_B200_UNITS": "1"}], ids=["unit-walk-forced"])
 def test_gpu_alternative_bodies_on_the_catalogue(env):
     e = dict(os.environ)
     e.update(env)

@@ -86,7 +86,7 @@ typedef int32_t i32;
 #define FLAG_VERIFY 1u
 #define FLAG_UNITS_ON 4u
 #define FLAG_UNITS_OFF 8u
-#define FLAG_DEFERRED 2u /* only jobs whose status says D2_DEFER (left over by the lean instance or zxc_decode2_kernel) */
+#define FLAG_DEFERRED 2u /* only jobs whose status says D2_DEFER (left over by the lean instance) */
 #define D2_DEFER_STATUS ((i32)0x80000000)
 
 struct DecodeParams {
@@ -103,7 +103,7 @@ struct DecodeParams {
     u32 scratch_stride;
     u32 flags;
     u32 block_cap; /* largest decoded block size of this launch: sizes the per-warp scratch regions */
-    u32* defer_list;  /* job indices the lean instance or zxc_decode2_kernel left to a FLAG_DEFERRED launch ... */
+    u32* defer_list;  /* job indices the lean instance left to a FLAG_DEFERRED launch ... */
     u32* defer_count; /* ... how many; more than defer_cap means "scan the status array instead" */
     u32 defer_cap;
 };

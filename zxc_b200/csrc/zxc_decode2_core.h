@@ -1,11 +1,10 @@
 /*
- * zxc_decode2_core.h -- integer core of the block-cooperative decode kernel (zxc_decode2.cuh).
+ * zxc_decode2_core.h -- integer helpers shared by the decode kernels (zxc_decode.cuh, zxc_decode_units.cuh):
  *
- * The kernel turns the reference's per-sequence loop (zxc_decompress.c:847-1209 GLO, :1231-1469 GHI)
- * inside out: instead of "for each sequence: copy ll literals, copy ml match bytes", every aligned
- * 4-byte OUTPUT word asks "which sequence covers me, and where do my bytes come from".  The
- * per-sequence facts that question needs are prepared once per block by a sequence-parallel pass
- * (prefix sums over ll / ll+ml, extras resolved) and stored as one 8-byte record per sequence:
+ *   - the extras-section segment-map scan, which resolves every varint of a block's extras section in one
+ *     warp-wide prefix scan instead of a serial walk;
+ *   - the 8-byte per-sequence record of the output-centric body (zxc_decode_units.cuh), which answers "which
+ *     sequence covers output position q, and where do its bytes come from":
  *
  *     w0 = (E - 1) | md << 16        E  = output position one past the sequence's last byte
  *                                    md = output position of its first match byte (literals end)
@@ -13,13 +12,8 @@
  *                                    (literal k of the run sits at literal-stream index q - M for
  *                                    output position q, so one delta serves the whole run)
  *
- * A word that lies inside one region (literal run or match) is one unaligned 4-byte gather; a word
- * cut by a region boundary merges two (rarely three) gathers.  Self-overlapping matches (off < ml,
- * :197-413 in the reference) read `md - off + (k mod off)`, i.e. only bytes in front of the match.
- *
- * Everything in this header is plain integer arithmetic shared by the device code and by the host
- * model test (oracle/decode2_model.cc, test infrastructure), which replays the kernel's two phases
- * sequentially and diffs against the reference.
+ *     Self-overlapping matches (off < ml, :197-413 in the reference) read `md - off + (k mod off)`, i.e. only
+ *     bytes in front of the match.
  */
 #ifndef ZXC_DECODE2_CORE_H
 #define ZXC_DECODE2_CORE_H
@@ -32,10 +26,7 @@
 #define Z2_HD static inline
 #endif
 
-#define Z2_WIN_MAX 65536u   /* largest decoded block the block-cooperative kernel takes */
-#define Z2_GROUP 512u       /* bytes of output one warp step produces (4 rows of 32 words) */
-#define Z2_ROWS 4u
-#define Z2_MD_INF 0x100000  /* "literals never end" for the virtual trailing-literal record */
+#define Z2_MD_INF 0x100000 /* "literals never end" for the virtual trailing-literal record */
 
 typedef struct {
     uint32_t w0, w1;
@@ -75,93 +66,6 @@ Z2_HD uint32_t z2_mod(uint32_t k, uint32_t off) {
     if (r < 0) r += (int32_t)off;
     if (r >= (int32_t)off) r -= (int32_t)off;
     return (uint32_t)r;
-}
-
-/* ---- the plan for one output word ------------------------------------------------------------
- * Positions are block-relative byte positions in the output window; a source position s >= 0 is
- * a window byte, s < 0 a dictionary byte (dict[dict_size + s]), literal sources are window
- * positions too (the literal stream is staged behind the output, at lit_pos + index).
- *   bytes [0, t)   come from srcX + b
- *   bytes [t, t2)  come from srcY + b
- *   bytes [t2, 4)  come from srcZ + b
- * need bit 0/1/2: region X/Y/Z is a match whose 4-byte source window must be complete first. */
-#define Z2_SLOW 8u /* byte-wise path: wrapped period, off < 4, dictionary source */
-
-typedef struct {
-    int32_t srcX, srcY, srcZ;
-    uint32_t t, t2;
-    uint32_t flags; /* need bits | Z2_SLOW */
-} z2_plan_t;
-
-Z2_HD z2_plan_t z2_word_plan(int32_t p, z2_seq_t c, z2_seq_t n, int32_t lit_pos) {
-    z2_plan_t pl;
-    pl.t = 4;
-    pl.t2 = 4;
-    pl.flags = 0;
-    const int32_t tA = c.md - p;
-    if (tA >= 4) { /* all literal */
-        pl.srcX = p + lit_pos - c.M;
-        pl.srcY = pl.srcX;
-        pl.srcZ = pl.srcX;
-        return pl;
-    }
-    if (tA > 0) { /* literal run ends inside the word, own match follows (>= 5 bytes: no third region) */
-        pl.srcX = p + lit_pos - c.M;
-        pl.t = (uint32_t)tA;
-        pl.srcY = p - c.off;
-        pl.srcZ = pl.srcY;
-        pl.flags = 2u;
-        if (c.off < 4 || pl.srcY < 0) pl.flags |= Z2_SLOW;
-        return pl;
-    }
-    /* word starts inside the match of `c` */
-    const int32_t k0 = p - c.md;
-    int32_t sx = p - c.off;
-    pl.flags = 1u;
-    if (k0 + 4 > c.off) { /* would read bytes of this very match: fold onto the period in front of it */
-        const uint32_t r0 = z2_mod((uint32_t)k0, (uint32_t)c.off);
-        if (c.off >= 4 && r0 + 4u <= (uint32_t)c.off) sx = c.md - c.off + (int32_t)r0;
-        else pl.flags |= Z2_SLOW;
-    }
-    if (sx < 0) pl.flags |= Z2_SLOW;
-    pl.srcX = sx;
-    pl.srcY = sx;
-    pl.srcZ = sx;
-    const int32_t tB = c.E - p;
-    if (tB >= 4) return pl;
-    pl.t = (uint32_t)tB;
-    const int32_t lln = n.md - c.E; /* next sequence's literal run */
-    if (lln > 0) {
-        pl.srcY = p + lit_pos - n.M;
-        if (tB + lln < 4) {
-            pl.t2 = (uint32_t)(tB + lln);
-            pl.srcZ = p - n.off;
-            pl.flags |= 4u;
-            if (n.off < 4 || pl.srcZ < 0) pl.flags |= Z2_SLOW;
-        } else {
-            pl.srcZ = pl.srcY;
-        }
-    } else {
-        pl.srcY = p - n.off;
-        pl.srcZ = pl.srcY;
-        pl.flags |= 2u;
-        if (n.off < 4 || pl.srcY < 0) pl.flags |= Z2_SLOW;
-    }
-    return pl;
-}
-
-/* byte-wise source of output position q (slow path): returns the source position and whether it
- * is a match byte (whose source must be complete) */
-Z2_HD int32_t z2_byte_source(int32_t q, z2_seq_t c, z2_seq_t n, int32_t lit_pos, int* is_match) {
-    const z2_seq_t s = (q < c.E) ? c : n;
-    if (q < s.md) {
-        *is_match = 0;
-        return q + lit_pos - s.M;
-    }
-    *is_match = 1;
-    const uint32_t k = (uint32_t)(q - s.md);
-    const uint32_t r = (k < (uint32_t)s.off) ? k : z2_mod(k, (uint32_t)s.off);
-    return s.md - s.off + (int32_t)r;
 }
 
 /* ---- extras section: segment maps ----------------------------------------------------------------

@@ -8,9 +8,6 @@
  *                       default (instances: sequence-centric or output-centric body, with / without dictionary);
  *                       without checksum verification its lean instance runs first and the general one decodes
  *                       what the lean one deferred (GHI blocks, Huffman sections)
- *   zxc_decode2_kernel  (zxc_decode2.cuh) one CTA per block of <= 64 KiB, window in shared memory, cp.async.bulk in
- *                       and out; only with ZXC_B200_DECODE_V2=1 (it measured 6.7x slower on the H100, DESIGN.md section 3c); what
- *                       it defers (entropy-coded sections, checksum verification) goes to zxc_decode_kernel
  * Encode: zxc_encode.cuh (levels 1-5), zxc_encode_opt.cuh (levels 6-7); the frame of a device-to-device compress
  * is assembled by zxc_assemble.cuh.
  * Dictionary training: zxc_train.cuh (zxg_train_* at the end of this file).
@@ -26,7 +23,6 @@
 #include "zxc_gpu.h"
 
 #include "zxc_decode.cuh"
-#include "zxc_decode2.cuh"
 #include "zxc_encode.cuh"
 #include "zxc_assemble.cuh"
 #include "zxc_dplan.cuh"
@@ -609,58 +605,13 @@ static int grid_for(u32 n_jobs) {
 /* per-warp scratch for expanded literal sections; 256 bytes of lead-in so word loads may start below it */
 static u32 scratch_stride_for(u32 block_size) { return scr_stride(block_size); }
 
-/* ---- block-cooperative kernel: launch geometry by block size ---------------------------------- */
-struct D2Config {
-    u32 win, gap, rcap, threads, smem, ctas_per_sm, spill_stride;
-};
-static int d2_enabled(void) {
-    static int cached = -1;
-    if (cached < 0) {
-        const char* e = getenv("ZXC_B200_DECODE_V2");
-        cached = (e && e[0] == '1') ? 1 : 0; /* off: measured slower than the warp-per-block kernel (DESIGN.md) */
-    }
-    return cached;
-}
-/* 1 when blocks of `block_size` decoded bytes go through zxc_decode2_kernel */
-static int d2_config(u32 block_size, D2Config* c) {
-    if (!d2_enabled() || block_size == 0 || block_size > Z2_WIN_MAX) return 0;
-    const u32 win = (block_size + Z2_GROUP - 1) & ~(Z2_GROUP - 1);
-    const u32 gap = win < 4096u ? win : 4096u;
-    const u32 nseq_max = block_size / 5u + 16u + 4u; /* zxc_common.c:142-144 */
-    const u32 fixed = d2_off_rec(win, gap) + 4u * 8u;
-    const u32 sm_total = 233472u; /* 228 KB per SM, 1 KB reserved per resident CTA */
-    u32 n = sm_total / (fixed + nseq_max * 8u + 1024u);
-    u32 rcap = nseq_max, spill = 0;
-    if (n < 2) { /* two blocks per SM: the tail of very long sequence lists lives in global memory */
-        n = 2;
-        rcap = (sm_total / 2u - 1024u - fixed) / 8u;
-        spill = nseq_max + 4u;
-    }
-    const u32 threads = win >= 32768u ? 256u : win >= 16384u ? 128u : 64u;
-    if (n > 32u) n = 32u;
-    if (n * threads > 2048u) n = 2048u / threads;
-    c->win = win;
-    c->gap = gap;
-    c->rcap = rcap;
-    c->threads = threads;
-    c->smem = d2_smem_bytes(win, gap, rcap);
-    c->ctas_per_sm = n;
-    c->spill_stride = spill;
-    return 1;
-}
-static size_t d2_spill_bytes(const D2Config* c) {
-    return (size_t)(g_sm_count > 0 ? g_sm_count : 132) * c->ctas_per_sm * c->spill_stride * sizeof(z2_rec_t);
-}
-
 #define SCRATCH_TAIL (sizeof(unsigned long long) * 4)
 #define DEFER_CAP (1u << 16) /* listed deferred jobs; beyond that the second launch scans the status array */
 
 extern "C" size_t zxc_b200_decode_scratch_size(uint32_t block_size) {
     if (zxg_init() != ZXC_OK) return 0;
     const size_t warps = (size_t)g_sm_count * DECODE_CTAS_MAX * WARPS_PER_CTA;
-    size_t n = warps * scratch_stride_for(block_size) + 512; /* room to align the regions behind it to 256 bytes */
-    D2Config c;
-    if (d2_config(block_size, &c)) n += d2_spill_bytes(&c) + 256;
+    const size_t n = warps * scratch_stride_for(block_size) + 512; /* room to align the regions behind it to 256 bytes */
     return n + (size_t)DEFER_CAP * 4 + SCRATCH_TAIL;
 }
 
@@ -704,91 +655,15 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
     if (warp_scratch > scratch_size) return ZXC_ERROR_MEMORY;
     if (!preset && cudaMemsetAsync(d_counter, 0, 3 * sizeof(unsigned long long), st) != cudaSuccess)
         return ZXC_B200_ERROR_CUDA;
-    /* deferred-job list behind the per-warp scratch (and the block-cooperative kernel's spill area); its counter is the
-     * third work counter.  A scratch too small for it leaves the list empty: the second launch scans the status array. */
-    size_t off = (warp_scratch + 255) & ~(size_t)255;
+    /* deferred-job list behind the per-warp scratch; its counter is the third work counter.  A scratch too small for it
+     * leaves the list empty: the second launch scans the status array. */
+    const size_t off =(warp_scratch + 255) & ~(size_t)255;
     P.defer_count = (u32*)(d_counter + 2);
     P.defer_cap = off + (size_t)DEFER_CAP * 4 <= scratch_size ? DEFER_CAP : 0u;
     P.defer_list = (u32*)((u8*)d_scratch + off);
-    D2Config c;
-    if (!verify && d2_config(block_size, &c)) {
-        /* launch 1: one CTA per block, window in shared memory; launch 2: whatever it deferred */
-        static int attr_done_smem = 0;
-        if (attr_done_smem < (int)c.smem) {
-            if (cudaFuncSetAttribute(zxc_decode2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 233472 - 1024) !=
-                cudaSuccess)
-                return ZXC_B200_ERROR_CUDA;
-            attr_done_smem = 233472;
-        }
-        Decode2Params Q;
-        Q.src = P.src;
-        Q.dst = P.dst;
-        Q.jobs = d_jobs;
-        Q.status = d_status;
-        Q.dict = P.dict;
-        Q.counter = d_counter;
-        Q.spill = NULL;
-        Q.n_jobs = n_jobs;
-        Q.dict_size = P.dict_size;
-        Q.win = c.win;
-        Q.gap = c.gap;
-        Q.rcap = c.rcap;
-        Q.spill_stride = c.spill_stride;
-        const u32 resident = (u32)(g_sm_count > 0 ? g_sm_count : 132) * c.ctas_per_sm;
-        const u32 grid2 = n_jobs < resident ? n_jobs : resident;
-        if (c.spill_stride) {
-            if (off + (size_t)grid2 * c.spill_stride * sizeof(z2_rec_t) > scratch_size) return ZXC_ERROR_MEMORY;
-            Q.spill = (z2_rec_t*)((u8*)d_scratch + off);
-            off = (off + d2_spill_bytes(&c) + 255) & ~(size_t)255;
-        }
-        /* the list moves behind the spill area */
-        P.defer_cap = off + (size_t)DEFER_CAP * 4 <= scratch_size ? DEFER_CAP : 0u;
-        P.defer_list = (u32*)((u8*)d_scratch + off);
-        Q.defer_count = P.defer_count;
-        Q.defer_cap = P.defer_cap;
-        Q.defer_list = P.defer_list;
-        Q.trace = NULL;
-        const int want_trace = getenv("ZXC_B200_D2_TRACE") != NULL; /* development: per-phase cycle counts */
-        if (want_trace && cudaMalloc((void**)&Q.trace, (size_t)n_jobs * 128) == cudaSuccess)
-            cudaMemsetAsync(Q.trace, 0, (size_t)n_jobs * 128, st);
-        zxc_decode2_kernel<<<grid2, c.threads, c.smem, st>>>(Q);
-        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-        if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
-        if (Q.trace) {
-            unsigned long long* h = (unsigned long long*)malloc((size_t)n_jobs * 128);
-            cudaStreamSynchronize(st);
-            cudaMemcpy(h, Q.trace, (size_t)n_jobs * 128, cudaMemcpyDeviceToHost);
-            double acc[6] = {0, 0, 0, 0, 0, 0};
-            u32 cnt = 0;
-            for (u32 i = 0; i < n_jobs; i++) {
-                const unsigned long long* t = h + (size_t)i * 8;
-                if (!t[6] || !t[5]) continue; /* deferred / raw / failed jobs leave the later stamps empty */
-                for (int q = 0; q < 6; q++) acc[q] += (double)(t[q + 1] - t[q]);
-                cnt++;
-            }
-            if (cnt)
-                fprintf(stderr, "d2 trace (%u blocks, mean cycles): header+issue %.0f | load wait %.0f | extras %.0f | records %.0f | "
-                                "words %.0f | drain %.0f\n", cnt, acc[0] / cnt, acc[1] / cnt, acc[2] / cnt, acc[3] / cnt,
-                        acc[4] / cnt, acc[5] / cnt);
-            double w[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            for (u32 i = 0; i < n_jobs; i++) {
-                const unsigned long long* t = h + (size_t)i * 8;
-                if (!t[6] || !t[5]) continue;
-                for (int q = 0; q < 8; q++) w[q] += (double)h[(size_t)n_jobs * 8 + (size_t)i * 8 + q];
-            }
-            if (cnt)
-                fprintf(stderr, "d2 trace warp 0 per block: steps %.1f rounds %.1f sleeps %.1f | cycles: guard %.0f plan %.0f rounds %.0f "
-                                "sleep %.0f finish %.0f\n", w[7] / cnt, w[5] / cnt, w[6] / cnt, w[0] / cnt, w[1] / cnt, w[2] / cnt,
-                        w[3] / cnt, w[4] / cnt);
-            free(h);
-            cudaFree(Q.trace);
-        }
-        P.flags |= FLAG_DEFERRED;
-        P.counter = d_counter + 1;
-    }
     /* the dictionary-free instance carries neither the dictionary pointer nor its source classification (zxc_decode.cuh) */
     const bool has_dict = P.dict != NULL && P.dict_size != 0;
-    if (!verify && !units && !(P.flags & FLAG_DEFERRED)) {
+    if (!verify && !units) {
         /* launch 1: the lean instance decodes the RAW blocks and the GLO blocks without Huffman sections and lists the
          * rest; launch 2 below: the general instance decodes the listed jobs (its warps exit at once when there are none) */
 #ifdef LEAN_CARVEOUT
@@ -834,8 +709,6 @@ static int launch_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* d
 static size_t launch_scratch_bytes(u32 n_jobs, u32 block_size) {
     size_t n = (size_t)grid_for(n_jobs) * WARPS_PER_CTA * scratch_stride_for(block_size);
     n = (n + 255) & ~(size_t)255;
-    D2Config c;
-    if (d2_config(block_size, &c) && c.spill_stride) n = (n + d2_spill_bytes(&c) + 255) & ~(size_t)255;
     return n + (size_t)DEFER_CAP * 4 + 256;
 }
 

@@ -68,7 +68,7 @@ __global__ void zxc_train_count_kernel(const u8* corpus, unsigned long long kgra
 __global__ void __launch_bounds__(TRN_CTA, 1) zxc_train_seg_kernel(const u8* corpus, unsigned long long corpus_size,
                                                                   unsigned long long stride, u32 n_starts, const u32* freq,
                                                                   TrainSeg* seg) {
-    extern __shared__ unsigned short s_freq[];
+    extern __shared__ __align__(128) unsigned short s_freq[]; /* 128: the shared layout this kernel has always had */
     trn_load_table(s_freq, freq);
     const u32 lane = threadIdx.x & 31;
     const u32 nwarps = gridDim.x * (blockDim.x >> 5);
@@ -145,7 +145,7 @@ __global__ void __launch_bounds__(TRN_CTA, 1) zxc_train_pick_kernel(const TrainS
                                                                    const unsigned short* hashes, const u32* chunk_first,
                                                                    u32 n_chunks, const u32* freq, u32 capacity,
                                                                    TrainPick* picks, u32* res) {
-    extern __shared__ unsigned short s_freq[];
+    extern __shared__ __align__(128) unsigned short s_freq[]; /* 128: the shared layout this kernel has always had */
     unsigned short* s_h = s_freq + TRN_HASH_SIZE;
     __shared__ u32 s_state[2]; /* picks, total */
     trn_load_table(s_freq, freq);
