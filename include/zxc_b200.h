@@ -162,6 +162,57 @@ ZXC_EXPORT int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, 
                                           const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
                                           int64_t* d_result, void* stream);
 
+/* ---- many device-resident frames in one call: zxc_b200_decompress_device over a batch ---- */
+/* one frame of a batch; the array of them lives in DEVICE memory */
+typedef struct {
+    const void* src;       /* the frame, device memory */
+    uint64_t src_size;
+    void* dst;             /* its output, device memory */
+    uint64_t dst_capacity;
+} zxc_b200_frame_t;
+
+/* Device scratch for one zxc_b200_decompress_device_batch call of at most max_frames frames whose dst_capacity values
+ * add up to at most max_total_capacity, with blocks of at most block_size bytes (0: bad block size, no device, more
+ * than 2^30 frames, or a table too large to plan).  It holds a job table of
+ * Jt = ceil(max_total_capacity / ZXC_BLOCK_SIZE_MIN) + 3 x max_frames entries: 28 bytes each for the plan and the
+ * split, and a window of 28 bytes each per launch slot (2 per block size from 4 KiB up to block_size: 10 at 64 KiB);
+ * about 170 bytes per frame; and the decode kernels' per-warp scratch for the full resident grid at block_size
+ * (on an H100, 132 SMs: 83 MiB at 4 KiB blocks, 732 MiB at 64 KiB, whatever the batch). */
+ZXC_EXPORT size_t zxc_b200_decompress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_capacity,
+                                                                uint32_t block_size);
+
+/* Decompresses n_frames independent frames on `stream`, asynchronously: d_frames[i] names frame i's bytes
+ * src[0 .. src_size) and its output dst[0 .. dst_capacity), all in device memory.  d_results[i] (one device int64
+ * per frame) becomes exactly what zxc_b200_decompress_device returns in *d_result for that frame with the same opts
+ * and a scratch of zxc_b200_decompress_device_scratch_size(dst_capacity, B), and dst[0 .. d_results[i]) equals its
+ * output; B is the block size the scratch was sized for (below).  The device also makes that call's host checks per
+ * frame, in zxc_decompress's order: ZXC_ERROR_NULL_INPUT for a NULL src, or a NULL dst with dst_capacity > 0, then
+ * ZXC_ERROR_SRC_TOO_SMALL for src_size below file header + footer.
+ * Returns ZXC_OK once enqueued, or a verdict for the whole call that replaces every frame's own (d_results is then
+ * not written), in this order: ZXC_ERROR_NULL_INPUT for a NULL d_frames, d_results or d_scratch when n_frames > 0;
+ * ZXC_ERROR_DICT_TOO_LARGE; ZXC_B200_ERROR_NO_DEVICE; ZXC_ERROR_MEMORY when scratch_size is below
+ * zxc_b200_decompress_device_batch_scratch_size(n_frames, 0, 4096).  n_frames == 0 returns ZXC_OK (after the
+ * dictionary and device checks) and launches nothing.
+ * The scratch: B is the largest block size whose layout with the smallest table (max_total_capacity 0) fits
+ * scratch_size, and the call then takes the largest job table that fits at B.  A scratch from
+ * zxc_b200_decompress_device_batch_scratch_size(n, C, b) gives B = b as long as the table's share of it is below the
+ * per-warp regions' step to 2b (C below about 2 GiB at 4 KiB blocks, 9 GiB at 64 KiB).  Frames take ceil(dst_capacity /
+ * ZXC_BLOCK_SIZE_MIN) + 2 table entries each, in index order (frames that fail the argument checks take none); from
+ * the first frame whose entries no longer fit the table, every later frame that passed the argument checks gets
+ * ZXC_ERROR_MEMORY and decodes nothing.  That happens only when the capacities add up to more than the
+ * max_total_capacity the scratch was sized for.
+ * Nothing outside the union of the frames' dst[0 .. dst_capacity), the scratch and d_results is written; overlapping
+ * outputs get unspecified bytes.  Reads of each src stay inside the bounds documented for zxc_b200_decompress_device.
+ * There is no host synchronisation and no allocation without a dictionary, and the call may then be captured in a
+ * CUDA graph; d_frames, the frames' bytes and d_results may change between replays.  A dictionary (one for the whole
+ * batch, host memory) is staged as in zxc_b200_decompress_device: a host copy, not capturable.  Kernel launches per
+ * call (zxc_b200_launch_count): 14 + k * (2 + c) whatever the frames, k and c as for zxc_b200_decompress_device with
+ * the B above (plan: 8; the decode kernels' lean and general instance per slot; check and decide: 2; the general
+ * split: 4, which exit at once when no frame needs it). */
+ZXC_EXPORT int zxc_b200_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
+                                                const zxc_decompress_opts_t* opts, void* d_scratch,
+                                                size_t scratch_size, int64_t* d_results, void* stream);
+
 /* ---- random access into a seekable frame in HBM: the device twin of zxc_seekable_open +
  *      zxc_seekable_decompress_range, for many ranges per call ---- */
 typedef struct zxc_b200_seekable_device_s zxc_b200_seekable_device;

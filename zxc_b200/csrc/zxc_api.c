@@ -991,6 +991,31 @@ int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst
                                  scratch_size, d_result, stream);
 }
 
+size_t zxc_b200_decompress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_capacity,
+                                                     uint32_t block_size) {
+    if (!zxf_valid_block_size(block_size)) return 0;
+    return zxg_decompress_batch_scratch_bytes(max_frames, max_total_capacity, block_size);
+}
+
+/* The host decides what needs neither the descriptors nor the frames' bytes; the device decides the rest per frame
+ * and writes it to d_results (zxc_dbatch.cuh). */
+int zxc_b200_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
+                                     const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                                     int64_t* d_results, void* stream) {
+    if (n_frames > 0 && (!d_frames || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
+    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
+    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    const int irc = zxg_init();
+    if (irc != ZXC_OK || n_frames == 0) return irc;
+    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
+    const int arc = dict_size ? dict_huf_attach(dict_huf) : 0;
+    return zxg_decompress_device_batch(d_frames, n_frames, dict_size ? dict : NULL, (uint32_t)dict_size,
+                                       arc == 1 ? dict_huf : NULL, did, arc, opts ? opts->checksum_enabled : 0,
+                                       d_scratch, scratch_size, d_results, stream);
+}
+
 int64_t zxc_compress_cctx(zxc_cctx* cctx, const void* src, size_t src_size, void* dst, size_t dst_capacity,
                           const zxc_compress_opts_t* opts) {
     if (!cctx) return ZXC_ERROR_NULL_INPUT;

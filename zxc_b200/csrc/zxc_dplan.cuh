@@ -103,7 +103,8 @@ __device__ __forceinline__ u32 dp_rotl(u32 v, u32 r) { return r ? (v << r) | (v 
 
 /* expected_block_bytes / decompress_frame's planned size of block i: block_size for every block but the last; the
  * last gets the footer's remainder (block_size when that is 0) */
-__device__ __forceinline__ u32 dp_planned(const DPlanState* S, u64 i, u64 n) {
+template <class St>
+__device__ __forceinline__ u32 dp_planned(const St* S, u64 i, u64 n) {
     const u32 bs = S->block_size;
     if (i + 1 < n) return bs;
     const u64 start = i * bs;
@@ -113,7 +114,8 @@ __device__ __forceinline__ u32 dp_planned(const DPlanState* S, u64 i, u64 n) {
 }
 
 /* decompress_frame's checks behind the decode (the `decoded:` label) */
-__device__ __forceinline__ long long dp_tail(const DPlanState* S, u64 produced, bool all_fit) {
+template <class St>
+__device__ __forceinline__ long long dp_tail(const St* S, u64 produced, bool all_fit) {
     if (!all_fit) return ZXC_ERROR_DST_TOO_SMALL;
     if (S->end == ZXW_END_BAD_HEADER) return ZXC_ERROR_BAD_HEADER;
     if (S->end == ZXW_END_EOF) {
@@ -125,10 +127,13 @@ __device__ __forceinline__ long long dp_tail(const DPlanState* S, u64 produced, 
 
 __device__ __forceinline__ void dp_prefetch(const u8* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
-__global__ void zxc_dplan_probe(const DPlanArgs A) {
-    DPlanState* S = A.st;
+/* zxc_dplan_probe's body for one frame of size >= header + footer; zxc_dbatch_probe runs it per frame too.  Ar has
+ * DPlanArgs's fields the probe reads, and its `st` points to a DPlanState or a DBatchFrame (one frame's plan). */
+template <class Ar>
+__device__ __forceinline__ void dp_probe(const Ar A) {
+    auto* S = A.st;
     const u8* s = A.src;
-    const u64 size = A.src_size; /* >= header + footer: checked on the host */
+    const u64 size = A.src_size; /* >= header + footer: checked before (on the host, or by zxc_dbatch_tiles) */
     S->done = S->fast = S->split = S->redecode = 0;
     S->hint_n = 0;
     S->ghash = 0;
@@ -180,6 +185,10 @@ __global__ void zxc_dplan_probe(const DPlanArgs A) {
             }
         }
     }
+}
+
+__global__ void zxc_dplan_probe(const DPlanArgs A) {
+    dp_probe(A);
 }
 
 __global__ void __launch_bounds__(ASM_THREADS) zxc_dplan_sek_tiles(const DPlanArgs A) {
@@ -272,12 +281,9 @@ __global__ void __launch_bounds__(ASM_THREADS) zxc_dplan_sek_blocks(const DPlanA
 /* zxw_walk, warp-uniform: every lane follows the chain (the header loads are broadcasts), lane 0 stores.  With a SEK
  * table the lanes prefetch the next 32 predicted headers into L2, a window ahead of the walk, like the host walk; a
  * wrong or forged table only prefetches the wrong lines. */
-__global__ void zxc_dplan_walk(const DPlanArgs A) {
-    DPlanState* S = A.st;
-    if (S->done || S->fast) return;
-    const u32 lane = threadIdx.x & 31;
-    const u8* s = A.src;
-    const u64 size = A.src_size;
+template <class St>
+__device__ __forceinline__ void dp_walk(const u8* s, const u64 size, zxc_b200_job_t* plan, const u32 J, St* S,
+                                        const u32 lane) {
     const u32 trailer = S->has_checksum ? ZXF_BLOCK_CKS : 0u;
     const u32 hint_n = S->hint_n;
     const u8* he = s + S->sek_pos;
@@ -307,13 +313,13 @@ __global__ void zxc_dplan_walk(const DPlanArgs A) {
             break;
         }
         const u64 on_disk = (u64)ZXF_BLOCK_HDR + comp + trailer;
-        if (lane == 0 && n < A.J) { /* beyond the table only the count matters (zxc_dplan_decide) */
+        if (lane == 0 && n < J) { /* beyond the table only the count matters (zxc_dplan_decide) */
             zxc_b200_job_t Jb;
             Jb.src_off = ip;
             Jb.dst_off = 0;
             Jb.src_len = (u32)(on_disk < rem ? on_disk : (rem > 0xFFFFFFFFull ? 0xFFFFFFFFull : rem));
             Jb.dst_cap = 0;
-            A.plan[n] = Jb;
+            plan[n] = Jb;
         }
         n++;
         if (trailer && on_disk <= rem) g = dp_rotl(g, 1) ^ ld32(s + ip + ZXF_BLOCK_HDR + comp);
@@ -324,6 +330,12 @@ __global__ void zxc_dplan_walk(const DPlanArgs A) {
     S->n = n;
     S->end = end;
     S->ghash = g;
+}
+
+__global__ void zxc_dplan_walk(const DPlanArgs A) {
+    DPlanState* S = A.st;
+    if (S->done || S->fast) return;
+    dp_walk(A.src, A.src_size, A.plan, A.J, S, threadIdx.x & 31);
 }
 
 /* regular plan: block i at i * block_size with its planned size, as far as dst_capacity goes */

@@ -25,6 +25,7 @@
 #include "zxc_decode.cuh"
 #include "zxc_encode.cuh"
 #include "zxc_assemble.cuh"
+#include "zxc_dbatch.cuh"
 #include "zxc_dplan.cuh"
 #include "zxc_dseek.cuh"
 #include "zxc_train.cuh"
@@ -1467,6 +1468,198 @@ extern "C" int zxg_decompress_device(const void* d_src, uint64_t src_size, void*
     if (has_dict) launch_dsplit<true>(D, 1, dec_grid, st);
     else launch_dsplit<false>(D, 1, dec_grid, st);
     zxc_dsplit_final<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* many device-resident frames in one call (zxc_b200_decompress_device_batch: */
+/* kernels in zxc_dbatch.cuh)                                                */
+/* ------------------------------------------------------------------------- */
+/* Scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned):
+ *   DBatchState | dictionary + its literal table | frames (n x DBatchFrame) | table offsets (n x u64) | tile sums |
+ *   slot tile sums (n_slots per tile) | plan (Jt jobs) | split sizes (Jt x i32) | slot windows (n_slots x Jt jobs) |
+ *   slot status (n_slots x Jt x i32) | split probe slots | decode scratch (per-warp regions, deferred list)
+ * n_slots = 2 per block size from 4 KiB up to B (checksum verification off / on).  The per-warp regions are sized for
+ * the full resident grid at B, whatever Jt: so B, which the call finds as the largest block size whose layout with
+ * the smallest table fits the scratch, is the block size the scratch was sized for unless the table's share is larger
+ * than the step in the per-warp regions to the next block size. */
+struct DBatchLayout {
+    size_t dict, frames, base, tiles, stiles, plan, sizes, jobs, status, slots, dec, dec_bytes, total;
+    u32 n_slots, probe_warps, room;
+    u64 Jt;
+};
+#define DB_J_MAX 0x7FFFFFFFull
+#define DB_FRAMES_MAX (1u << 30)
+
+static void db_layout(u32 n, u64 Jt, u32 bs, DBatchLayout* L) {
+    const size_t n_tiles = ((size_t)n + ASM_TILE - 1) / ASM_TILE;
+    L->n_slots = ((u32)__builtin_ctz(bs) - ZXC_BLOCK_SIZE_MIN_LOG2 + 1) * 2;
+    size_t o = DB_STATE_BYTES;
+    L->dict = o;
+    o += r256((size_t)ZXC_DICT_SIZE_MAX + ZXC_HUF_TABLE_SIZE);
+    L->frames = o;
+    o += r256((size_t)n * sizeof(DBatchFrame));
+    L->base = o;
+    o += r256((size_t)n * 8);
+    L->tiles = o;
+    o += r256(n_tiles * 8);
+    L->stiles = o;
+    o += r256(n_tiles * L->n_slots * 8);
+    L->plan = o;
+    o += r256((size_t)Jt * sizeof(zxc_b200_job_t));
+    L->sizes = o;
+    o += r256((size_t)Jt * 4);
+    L->jobs = o;
+    o += r256((size_t)L->n_slots * Jt * sizeof(zxc_b200_job_t));
+    L->status = o;
+    o += r256((size_t)L->n_slots * Jt * 4);
+    /* the split's size probe: one slot of bs + ZXF_TAIL_PAD per warp, at most 256 MiB of them (a rare path) */
+    L->room = bs + ZXF_TAIL_PAD;
+    const u32 dec_warps = (u32)grid_for((u32)DB_J_MAX) * WARPS_PER_CTA;
+    const u32 by_room = (u32)(((size_t)256 << 20) / L->room);
+    u64 pw = dec_warps < by_room ? dec_warps : by_room;
+    if (pw > Jt) pw = Jt;
+    L->probe_warps = pw ? (u32)pw : 1;
+    L->slots = o;
+    o += r256((size_t)L->probe_warps * L->room);
+    L->dec = o;
+    L->dec_bytes = launch_scratch_bytes((u32)DB_J_MAX, bs);
+    L->total = o + L->dec_bytes + 256; /* base alignment slack */
+    L->Jt = Jt;
+}
+
+extern "C" size_t zxg_decompress_batch_scratch_bytes(uint32_t max_frames, uint64_t max_total_capacity,
+                                                     uint32_t block_size) {
+    if (zxg_init() != ZXC_OK || max_frames > DB_FRAMES_MAX) return 0;
+    const u64 Jt = max_total_capacity / ZXC_BLOCK_SIZE_MIN + (max_total_capacity % ZXC_BLOCK_SIZE_MIN != 0) +
+                   3ull * max_frames;
+    if (Jt > DB_J_MAX) return 0;
+    DBatchLayout L;
+    db_layout(max_frames, Jt ? Jt : 1, block_size, &L);
+    return L.total;
+}
+
+template <bool HAS_DICT>
+static void launch_dbatch_split(const DBatchSplitArgs& D, u32 phase, u32 grid, cudaStream_t st) {
+    zxc_dbatch_split<HAS_DICT><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(D, phase);
+}
+
+extern "C" int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const void* h_dict,
+                                           uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id,
+                                           int huf_verdict, int checksum_enabled, void* d_scratch,
+                                           size_t scratch_size, int64_t* d_results, void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    const u32 n = n_frames;
+    if (n > DB_FRAMES_MAX) return ZXC_ERROR_MEMORY;
+    const u64 J_min = 3ull * n;
+    /* the largest block size whose layout with the smallest table fits, then the largest table at it */
+    u32 bs = 0;
+    DBatchLayout L;
+    for (u32 b = ZXC_BLOCK_SIZE_MAX; b >= ZXC_BLOCK_SIZE_MIN; b >>= 1) {
+        db_layout(n, J_min, b, &L);
+        if (L.total <= scratch_size) {
+            bs = b;
+            break;
+        }
+    }
+    if (!bs) return ZXC_ERROR_MEMORY;
+    u64 lo = J_min, hi = DB_J_MAX;
+    while (lo < hi) {
+        const u64 mid = lo + (hi - lo + 1) / 2;
+        db_layout(n, mid, bs, &L);
+        if (L.total <= scratch_size) lo = mid;
+        else hi = mid - 1;
+    }
+    db_layout(n, lo, bs, &L);
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    const bool has_dict = h_dict && dict_size;
+    u8* d_dict = NULL;
+    u8* d_huf = NULL;
+    if (has_dict) { /* staged as in zxg_decompress_device */
+        d_dict = base + L.dict;
+        const size_t dbytes = (size_t)dict_size + (h_dict_huf ? ZXC_HUF_TABLE_SIZE : 0);
+        u8* b = (u8*)host_bounce(h_dict, dict_size, dbytes);
+        if (!b) return ZXC_ERROR_MEMORY;
+        if (h_dict_huf) {
+            memcpy(b + dict_size, h_dict_huf, ZXC_HUF_TABLE_SIZE);
+            d_huf = d_dict + dict_size;
+        }
+        const cudaError_t e = cudaMemcpyAsync(d_dict, b, dbytes, cudaMemcpyHostToDevice, st);
+        free(b);
+        if (e != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    }
+    DBatchState* S = (DBatchState*)base;
+    DBatchArgs A;
+    A.frames = d_frames;
+    A.results = (long long*)d_results;
+    A.st = S;
+    A.F = (DBatchFrame*)(base + L.frames);
+    A.base = (unsigned long long*)(base + L.base);
+    A.tiles = (unsigned long long*)(base + L.tiles);
+    A.stiles = (unsigned long long*)(base + L.stiles);
+    A.plan = (zxc_b200_job_t*)(base + L.plan);
+    A.sizes = (i32*)(base + L.sizes);
+    A.jobs = (zxc_b200_job_t*)(base + L.jobs);
+    A.status = (i32*)(base + L.status);
+    A.Jt = L.Jt;
+    A.n = n;
+    A.n_slots = L.n_slots;
+    A.max_block_size = bs;
+    A.dict_id = dict_id;
+    A.have_dict = has_dict ? 1u : 0u;
+    A.huf_verdict = huf_verdict;
+    A.checksum_enabled = checksum_enabled ? 1u : 0u;
+    const u32 n_tiles = (n + ASM_TILE - 1) / ASM_TILE;
+    const u32 per_frame = (n + DB_THREADS - 1) / DB_THREADS;
+    const u32 per_cta = n < 4096 ? n : 4096; /* grid-stride over frames, one CTA each */
+    const u64 by_entry = (L.Jt + DB_THREADS - 1) / DB_THREADS;
+    const u32 per_entry = (u32)(by_entry < 16384 ? by_entry : 16384);
+    zxc_dbatch_tiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dbatch_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_dbatch_probe<<<per_frame, DB_THREADS, 0, st>>>(A);
+    zxc_dbatch_sek<<<per_cta, ASM_THREADS, 0, st>>>(A);
+    zxc_dbatch_walk<<<(u32)(((u64)n * 32 + DB_THREADS - 1) / DB_THREADS), DB_THREADS, 0, st>>>(A);
+    zxc_dbatch_count<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dbatch_slots<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_dbatch_place<<<per_entry, DB_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 8, __ATOMIC_RELAXED);
+    if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    /* one launch slot per block size up to bs, and per checksum verification off / on, each over its own window */
+    u8* dec = base + L.dec;
+    for (u32 b = ZXC_BLOCK_SIZE_MIN; b <= bs; b <<= 1) {
+        const u32 lg = (u32)__builtin_ctz(b) - ZXC_BLOCK_SIZE_MIN_LOG2;
+        for (int v = 0; v <= (checksum_enabled ? 1 : 0); v++) {
+            const u32 slot = lg * 2 + v;
+            const int rc = launch_decode(NULL, NULL, A.jobs + slot * L.Jt, (u32)L.Jt, A.status + slot * L.Jt, d_dict,
+                                         dict_size, d_huf, dec, L.dec_bytes, b, v, S->ctr[slot], st, 1);
+            if (rc != ZXC_OK) return rc;
+        }
+    }
+    zxc_dbatch_check<<<per_entry, DB_THREADS, 0, st>>>(A);
+    zxc_dbatch_decide<<<per_frame, DB_THREADS, 0, st>>>(A);
+    DBatchSplitArgs D;
+    D.a = A;
+    D.zero = NULL;
+    D.slots = base + L.slots;
+    D.scratch = dec;
+    D.dict = d_dict;
+    D.dict_huf = d_huf;
+    D.dict_size = has_dict ? dict_size : 0;
+    D.scratch_stride = scratch_stride_for(bs);
+    D.room = L.room;
+    D.probe_warps = L.probe_warps;
+    const u32 probe_grid = (L.probe_warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
+    const u32 dec_grid = (u32)grid_for((u32)L.Jt);
+    const u32 split_ctas = n < 1024 ? n : 1024;
+    if (has_dict) launch_dbatch_split<true>(D, 0, probe_grid, st);
+    else launch_dbatch_split<false>(D, 0, probe_grid, st);
+    zxc_dbatch_split_scan<<<split_ctas, ASM_SCAN_THREADS, 0, st>>>(A);
+    if (has_dict) launch_dbatch_split<true>(D, 1, dec_grid, st);
+    else launch_dbatch_split<false>(D, 1, dec_grid, st);
+    zxc_dbatch_split_final<<<split_ctas, ASM_SCAN_THREADS, 0, st>>>(A);
     __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }

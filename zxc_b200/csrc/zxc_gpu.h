@@ -82,6 +82,16 @@ int zxg_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uin
                           int huf_verdict, int checksum_enabled, void* d_scratch, size_t scratch_size,
                           int64_t* d_result, void* stream);
 
+/* Many device-resident frames in one call (zxc_b200_decompress_device_batch; kernels in zxc_dbatch.cuh), with the
+ * host's share of the verdicts made as for zxg_decompress_device.  Scratch for up to max_frames frames of at most
+ * max_total_capacity output bytes in all and block_size-byte blocks (0 without a device or when that cannot be
+ * planned); ZXC_ERROR_MEMORY when the scratch holds less than that for no output and 4 KiB blocks. */
+size_t zxg_decompress_batch_scratch_bytes(uint32_t max_frames, uint64_t max_total_capacity, uint32_t block_size);
+int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const void* h_dict,
+                                uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id, int huf_verdict,
+                                int checksum_enabled, void* d_scratch, size_t scratch_size, int64_t* d_results,
+                                void* stream);
+
 /* Device-resident seekable frames (zxc_dseek.c; kernels in zxc_dseek.cuh).  What a range call needs of its handle. */
 typedef struct {
     const void* d_src;

@@ -4,7 +4,8 @@
 through the host.  ``decompress`` decodes such a frame with zxc_b200_decode_blocks from the decode plan the
 compress call emitted.  ``decompress_frame`` decodes any frame held in a uint8 CUDA tensor with
 zxc_b200_decompress_device, which plans, decodes and checks it on the device.  ``SeekableFrame`` decodes byte ranges of
-a seekable frame in HBM with zxc_b200_seekable_device_decompress_ranges.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
+a seekable frame in HBM with zxc_b200_seekable_device_decompress_ranges.  ``decompress_frames`` decodes many frames
+in one zxc_b200_decompress_device_batch call.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
 """
 import ctypes as C
 from dataclasses import dataclass
@@ -218,6 +219,110 @@ def decompress_frame(frame, *, capacity=None, dict=None, dict_huf=None, checksum
     if r < 0:
         raise ZxcError(r, "zxc_b200_decompress_device")
     return out[:r]
+
+
+lib.zxc_b200_decompress_device_batch_scratch_size.restype = C.c_size_t
+lib.zxc_b200_decompress_device_batch_scratch_size.argtypes = [C.c_uint32, C.c_uint64, C.c_uint32]
+lib.zxc_b200_decompress_device_batch.restype = C.c_int
+lib.zxc_b200_decompress_device_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                 C.c_void_p, C.c_void_p]
+
+
+def decompress_frames(frames, capacities=None, *, out=None, dict=None, dict_huf=None, checksum=False, block_size=None,
+                      stream=None):
+    """Decode many ZXC frames, each a contiguous uint8 CUDA tensor on one device, in one batch call.
+
+    Returns (outs, results): outs[i] is frame i's output tensor, results an int64 CUDA tensor where results[i] is
+    exactly what decompress_frame's zxc_b200_decompress_device call gives frame i (its byte count or a negative
+    zxc_error_t code; the bytes of a failed frame are unspecified).  capacities gives each frame's output room; with
+    capacities=None every frame's footer and header byte are read with one gathered device-to-host copy, sized with
+    decompress_frame's plausibility rule (ValueError for a footer past it, or a frame below 28 bytes).  `out`, a list
+    of contiguous uint8 tensors on the frames' device, one per frame, takes the outputs instead (its sizes are the
+    capacities).  block_size is the largest block size to accept (frames with larger blocks get ZXC_ERROR_MEMORY, as
+    zxc_b200_decompress_device with a scratch sized for it gives): by default the largest any frame's header names
+    when capacities are read from the footers, else 64 KiB.  The work runs on `stream` (default: the current stream), which first waits for the current stream; with `out` or
+    capacities given nothing synchronises.  Argument errors raise ValueError before anything is enqueued; a rejected
+    call raises ZxcError.  dict / dict_huf are host bytes, one dictionary for the batch."""
+    frames = list(frames)
+    if not frames:
+        raise ValueError("frames is empty")
+    dev = frames[0].device
+    for f in frames:
+        if not f.is_cuda or f.dtype != torch.uint8 or not f.is_contiguous():
+            raise ValueError("every frame must be a contiguous uint8 CUDA tensor")
+        if f.device != dev:
+            raise ValueError(f"every frame must be on {dev}, not {f.device}")
+    frames = [f.reshape(-1) for f in frames]
+    n = len(frames)
+    if out is not None:
+        out = list(out)
+        if len(out) != n:
+            raise ValueError("out must hold one tensor per frame")
+        for o in out:
+            _check_out(o, dev)
+        if capacities is not None and [int(c) for c in capacities] != [o.numel() for o in out]:
+            raise ValueError("capacities differ from the sizes of out")
+        capacities = [o.numel() for o in out]
+    if block_size is not None and block_size not in [1 << k for k in range(12, 22)]:
+        raise ValueError("block_size must be a power of two from 4 KiB to 2 MiB")
+    if capacities is not None:
+        block_size = block_size or 65536
+        capacities = [int(c) for c in capacities]
+        if len(capacities) != n:
+            raise ValueError("capacities must hold one value per frame")
+        if any(c < 0 for c in capacities):
+            raise ValueError("capacities must not be negative")
+    o = _DOpts(checksum_enabled=int(bool(checksum)))
+    keep = []
+    if dict is not None:
+        d = bytes(dict)
+        keep.append(d)
+        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+        if dict_huf is not None:
+            h = bytes(dict_huf)
+            keep.append(h)
+            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    with torch.cuda.device(dev):
+        current = torch.cuda.current_stream(dev)
+        stream = stream or current
+        if stream != current:
+            # the inputs were made (or written) on the current stream; the caller may drop them on return
+            stream.wait_stream(current)
+            for t in frames + (out or []):
+                t.record_stream(stream)
+        with torch.cuda.stream(stream):
+            if capacities is None:
+                # one gathered copy: every frame's header block-size byte and 8-byte footer
+                sizes = [f.numel() for f in frames]
+                if min(sizes) < 28:
+                    raise ValueError("a frame below 28 bytes has no footer; pass capacities")
+                h = torch.cat([t for f in frames for t in (f[5:6], f[-12:-4])]).cpu().numpy().reshape(n, 9)
+                capacities, bs = [], 4096
+                for i, row in enumerate(h):
+                    b = 1 << int(row[0]) if 12 <= row[0] <= 21 else 4096
+                    footer = int.from_bytes(row[1:].tobytes(), "little")
+                    if -(-footer // b) > sizes[i] // 8:  # zxf_dsize_plausible
+                        raise ValueError(f"frame {i}'s footer claims {footer} bytes, more than it can hold; "
+                                         "pass capacities")
+                    capacities.append(footer)
+                    bs = max(bs, b)
+                block_size = block_size or bs
+            if out is None:
+                out = [torch.empty(max(c, 1), dtype=torch.uint8, device=dev)[:c] for c in capacities]
+            # page-locked, so the upload does not wait for the stream (the host allocator keeps it until it ran)
+            desc = torch.tensor([[f.data_ptr(), f.numel(), t.data_ptr() if c else 0, c]
+                                 for f, t, c in zip(frames, out, capacities)], dtype=torch.int64)
+            desc = desc.pin_memory().to(dev, non_blocking=True)
+            scratch_size = int(lib.zxc_b200_decompress_device_batch_scratch_size(n, sum(capacities), block_size))
+            if scratch_size == 0:
+                raise ValueError("zxc_b200_decompress_device_batch_scratch_size: too many frames or bytes, or no device")
+            scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
+            results = torch.empty(n, dtype=torch.int64, device=dev)
+            rc = lib.zxc_b200_decompress_device_batch(desc.data_ptr(), n, C.byref(o), scratch.data_ptr(),
+                                                      scratch_size, results.data_ptr(), stream.cuda_stream)
+            if rc != 0:
+                raise ZxcError(rc, "zxc_b200_decompress_device_batch")
+    return out, results
 
 
 lib.zxc_b200_seekable_device_open.restype = C.c_void_p
