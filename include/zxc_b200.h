@@ -213,6 +213,55 @@ ZXC_EXPORT int zxc_b200_decompress_device_batch(const zxc_b200_frame_t* d_frames
                                                 const zxc_decompress_opts_t* opts, void* d_scratch,
                                                 size_t scratch_size, int64_t* d_results, void* stream);
 
+/* ---- many device-resident buffers in one call: zxc_b200_compress_device over a batch ---- */
+/* Device scratch for one zxc_b200_compress_device_batch call of at most max_frames buffers whose src_size values add
+ * up to at most max_total_src, at these options (0: invalid options, no device, more than 2^30 buffers, or more than
+ * 2^50 bytes).  It holds about 112 bytes per buffer; a pool with each buffer's share (below); 12 bytes per block the
+ * pool can hold; and one encode slot per warp (zxc_b200_encode_scratch_size's per-warp share) for the full resident
+ * grid, or for one warp per block the pool can hold when that is fewer.  On an H100 (132 SMs, 4 224 warps), 4 096
+ * buffers of 64 KiB take about 2.8 GB at level 3 and 6.1 GB at level 6. */
+ZXC_EXPORT size_t zxc_b200_compress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_src,
+                                                              const zxc_compress_opts_t* opts);
+
+/* Compresses n_frames independent buffers on `stream`, asynchronously, into one ZXC frame each: d_frames[i] (device
+ * memory) names buffer i's bytes src[0 .. src_size) and its frame's room dst[0 .. dst_capacity), all in device memory.
+ * d_results[i] (one device int64 per buffer) becomes exactly what zxc_b200_compress_device gives that buffer alone in
+ * *d_result with the same opts, and dst[0 .. d_results[i]) equals its frame, so both equal zxc_compress's result and
+ * bytes.  One set of opts applies to the whole batch: level, block_size, checksum_enabled, seekable and one dictionary
+ * in HOST memory (read before the call returns, as for zxc_b200_compress_device).
+ * Per buffer, the device makes zxc_b200_compress_device's host checks in its order: ZXC_ERROR_NULL_INPUT for a NULL
+ * dst, dst_capacity 0, or a NULL src with src_size > 0; ZXC_ERROR_BAD_BLOCK_SIZE for more than 2^32 - 3 blocks;
+ * ZXC_ERROR_DST_TOO_SMALL for dst_capacity below header + trailer (which depends on the block count and seekable).
+ * Then the pool rule below (ZXC_ERROR_MEMORY), and last ZXC_ERROR_DST_TOO_SMALL for a frame whose body does not fit
+ * (dst is then left untouched).
+ * Returns ZXC_OK once enqueued, or a verdict for the whole call that replaces every buffer's own (d_results is then
+ * not written), in zxc_b200_compress_device's order: ZXC_ERROR_NULL_INPUT for a NULL d_frames, d_results or d_scratch
+ * when n_frames > 0; ZXC_ERROR_DICT_TOO_LARGE; ZXC_ERROR_BAD_BLOCK_SIZE from the options; ZXC_B200_ERROR_NO_DEVICE;
+ * ZXC_ERROR_CORRUPT_DATA for a malformed dict_huf; ZXC_ERROR_MEMORY when scratch_size is below
+ * zxc_b200_compress_device_batch_scratch_size(n_frames, 0, opts).  n_frames == 0 returns ZXC_OK after those option,
+ * dictionary and device checks and launches nothing.
+ * The scratch: past about 112 bytes per buffer and the dictionary comes the room: a pool of P bytes, then one encode
+ * slot.  A non-empty buffer's share of the pool is its padded input copy, r256(src_size + 64) bytes, plus one staging
+ * slot of r256(block_size + 80) bytes per block; an empty buffer takes none.  Buffers take their shares in index order;
+ * from the first buffer whose share no longer fits, every later buffer that passed the checks gets ZXC_ERROR_MEMORY
+ * and nothing is written for it.  P is a function of (scratch_size, n_frames, opts) alone: the largest pool whose
+ * layout fits, where the layout holds, beside the room, a 4-byte size and an 8-byte offset for each of the
+ * nb_max = max(1, P / (r256(block_size + 80) + 256)) blocks such a pool can hold.  The encode runs up to
+ * W = min(resident encode grid, nb_max) warps (rounded down to a multiple of 4 from 4 up), one encode slot each,
+ * counted down from the room's end: every slot that fits in the part of the room the batch's shares leave free runs a
+ * warp, so a scratch from zxc_b200_compress_device_batch_scratch_size(n, T, opts) gives any batch of at most n
+ * buffers of at most T bytes no ZXC_ERROR_MEMORY and W warps, and a smaller one that still holds the shares runs fewer
+ * warps (down to one: same output, slower).
+ * Nothing outside [src, src + src_size) of each buffer is read, whatever its alignment; nothing outside the union of
+ * the dst[0 .. dst_capacity), the scratch and d_results is written, and overlapping outputs get unspecified bytes.
+ * There is no host synchronisation, no copy through the host and no allocation without a dictionary, and the call may
+ * then be captured in a CUDA graph; d_frames, the buffers' bytes and d_results may change between replays.  Kernel
+ * launches per call (zxc_b200_launch_count): 12 whatever the buffers (plan: 3; gather; encode; assembly: 5;
+ * compaction; finish), plus one dictionary-seeding kernel with a dictionary. */
+ZXC_EXPORT int zxc_b200_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
+                                              const zxc_compress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                                              int64_t* d_results, void* stream);
+
 /* ---- random access into a seekable frame in HBM: the device twin of zxc_seekable_open +
  *      zxc_seekable_decompress_range, for many ranges per call ---- */
 typedef struct zxc_b200_seekable_device_s zxc_b200_seekable_device;

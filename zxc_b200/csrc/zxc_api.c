@@ -966,6 +966,45 @@ int zxc_b200_compress_device(const void* d_src, uint64_t src_size, void* d_dst, 
                                d_jobs, stream);
 }
 
+size_t zxc_b200_compress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_src,
+                                                   const zxc_compress_opts_t* opts) {
+    int level;
+    size_t bs;
+    uint32_t nb;
+    if (device_opts(0, opts, &level, &bs, &nb) != ZXC_OK) return 0;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    return zxg_compress_batch_scratch_bytes(max_frames, max_total_src, (uint32_t)bs, level, (uint32_t)dict_size);
+}
+
+/* The host decides what needs no descriptor, in zxc_b200_compress_device's order; the device makes that call's
+ * per-buffer checks and the rest per frame and writes them to d_results (zxc_cbatch.cuh). */
+int zxc_b200_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const zxc_compress_opts_t* opts,
+                                   void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+    if (n_frames > 0 && (!d_frames || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
+    int level;
+    size_t block_size;
+    uint32_t nb;
+    int rc = device_opts(0, opts, &level, &block_size, &nb);
+    if (rc != ZXC_OK) return rc;
+    rc = zxg_init();
+    if (rc != ZXC_OK) return rc;
+    const int checksum = opts ? opts->checksum_enabled : 0;
+    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
+    uint8_t huf_lens[256];
+    int have_huf = 0;
+    rc = unpack_dict_huf(dict_huf, huf_lens, &have_huf);
+    if (rc != ZXC_OK || n_frames == 0) return rc;
+    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
+    uint8_t header[16], eof[8];
+    zxf_write_file_header(header, sizeof header, block_size, checksum, did);
+    zxf_write_block_header(eof, sizeof eof, ZXF_BT_EOF, 0);
+    return zxg_compress_device_batch(d_frames, n_frames, (uint32_t)block_size, level, checksum,
+                                     opts ? opts->seekable : 0, dict, (uint32_t)dict_size, have_huf ? huf_lens : NULL,
+                                     header, eof, d_scratch, scratch_size, d_results, stream);
+}
+
 size_t zxc_b200_decompress_device_scratch_size(uint64_t dst_capacity, uint32_t block_size) {
     if (!zxf_valid_block_size(block_size)) return 0;
     return zxg_decompress_scratch_bytes(dst_capacity, block_size);

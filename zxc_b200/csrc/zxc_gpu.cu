@@ -9,7 +9,7 @@
  *                       without checksum verification its lean instance runs first and the general one decodes
  *                       what the lean one deferred (GHI blocks, Huffman sections)
  * Encode: zxc_encode.cuh (levels 1-5), zxc_encode_opt.cuh (levels 6-7); the frame of a device-to-device compress
- * is assembled by zxc_assemble.cuh.
+ * is assembled by zxc_assemble.cuh, and a batch of them is encoded and assembled by zxc_cbatch.cuh.
  * Dictionary training: zxc_train.cuh (zxg_train_* at the end of this file).
  */
 #include <cuda_runtime.h>
@@ -26,6 +26,7 @@
 #include "zxc_encode.cuh"
 #include "zxc_assemble.cuh"
 #include "zxc_dbatch.cuh"
+#include "zxc_cbatch.cuh"
 #include "zxc_dplan.cuh"
 #include "zxc_dseek.cuh"
 #include "zxc_train.cuh"
@@ -1094,6 +1095,33 @@ struct EncLaunch {
     u32 dict_size;
     const uint8_t* h_dict_huf_lens;
 };
+/* The dictionary region of an encode at d_dict (enc_dict_bytes(dict_size) bytes): the host dictionary, read through a
+ * pageable copy (host_bounce) so the call has read it when it returns, and at level 6-7 the literal lengths, copied in;
+ * the match tables seeded by zxc_seed_kernel (one launch).  Fills P's dictionary fields. */
+static void* host_bounce(const void* p, size_t n, size_t bytes);
+static int enc_stage_dict(EncodeParams& P, u8* d_dict, const void* h_dict, u32 dict_size, int level,
+                          const uint8_t* h_dict_huf_lens, cudaStream_t st) {
+    void* bd = host_bounce(h_dict, dict_size, dict_size);
+    if (!bd) return ZXC_ERROR_MEMORY;
+    const size_t dpad = enc_dict_pad(dict_size);
+    const bool ok = cudaMemsetAsync(d_dict, 0, enc_dict_bytes(dict_size), st) == cudaSuccess &&
+                    cudaMemcpyAsync(d_dict, bd, dict_size, cudaMemcpyHostToDevice, st) == cudaSuccess;
+    free(bd);
+    if (!ok) return ZXC_B200_ERROR_CUDA;
+    P.dict = d_dict;
+    P.seed_head = (const u32*)(d_dict + dpad);
+    P.seed_chain = (const unsigned short*)(d_dict + dpad + (size_t)ENC_HASH_SIZE * 4);
+    if (h_dict_huf_lens && level >= 6) { /* the shared literal table, one length per byte */
+        u8* d_lens = d_dict + dpad + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2;
+        if (cudaMemcpyAsync(d_lens, h_dict_huf_lens, 256, cudaMemcpyHostToDevice, st) != cudaSuccess)
+            return ZXC_B200_ERROR_CUDA;
+        P.dict_huf_lens = d_lens;
+    }
+    zxc_seed_kernel<<<1, 32, 0, st>>>(d_dict, dict_size, (u32)level, (u32*)P.seed_head, (unsigned short*)P.seed_chain);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return ZXC_OK;
+}
+
 static int launch_encode(const EncLaunch& E, cudaStream_t st) {
     EncodeParams P;
     P.src = E.d_src;
@@ -1106,22 +1134,8 @@ static int launch_encode(const EncLaunch& E, cudaStream_t st) {
     P.seed_chain = NULL;
     P.dict_huf_lens = NULL;
     if (E.h_dict && E.dict_size) {
-        u8* d_dict = E.d_dict;
-        const size_t dpad = enc_dict_pad(E.dict_size);
-        if (cudaMemsetAsync(d_dict, 0, enc_dict_bytes(E.dict_size), st) != cudaSuccess ||
-            cudaMemcpyAsync(d_dict, E.h_dict, E.dict_size, cudaMemcpyHostToDevice, st) != cudaSuccess)
-            return ZXC_B200_ERROR_CUDA;
-        P.dict = d_dict;
-        P.seed_head = (const u32*)(d_dict + dpad);
-        P.seed_chain = (const unsigned short*)(d_dict + dpad + (size_t)ENC_HASH_SIZE * 4);
-        if (E.h_dict_huf_lens && E.level >= 6) { /* the shared literal table, one length per byte */
-            u8* d_lens = d_dict + dpad + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2;
-            if (cudaMemcpyAsync(d_lens, E.h_dict_huf_lens, 256, cudaMemcpyHostToDevice, st) != cudaSuccess)
-                return ZXC_B200_ERROR_CUDA;
-            P.dict_huf_lens = d_lens;
-        }
-        zxc_seed_kernel<<<1, 32, 0, st>>>(d_dict, E.dict_size, (u32)E.level, (u32*)P.seed_head, (unsigned short*)P.seed_chain);
-        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+        const int rc = enc_stage_dict(P, E.d_dict, E.h_dict, E.dict_size, E.level, E.h_dict_huf_lens, st);
+        if (rc != ZXC_OK) return rc;
     }
     P.src_size = E.src_size;
     P.scratch_stride = enc_layout(E.block_size, E.level).total;
@@ -1298,13 +1312,9 @@ extern "C" int zxg_compress_device(const void* d_src, uint64_t src_size, void* d
         if (cudaMemcpyAsync(d_in, d_src, (size_t)src_size, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
             cudaMemsetAsync(d_in + src_size, 0, 64, st) != cudaSuccess)
             return ZXC_B200_ERROR_CUDA;
-        /* the dictionary is read before the call returns, whatever memory the caller's is in (host_bounce) */
-        void* bd = NULL;
-        if (h_dict && dict_size && !(bd = host_bounce(h_dict, dict_size, dict_size))) return ZXC_ERROR_MEMORY;
         const EncLaunch E = {d_in, src_size, block_size, n_blocks, level, checksum, d_stage, d_sizes, base + L.warps,
-                             warps, &state->counter, base + L.dict, bd, dict_size, h_dict_huf_lens};
+                             warps, &state->counter, base + L.dict, h_dict, dict_size, h_dict_huf_lens};
         const int rc = launch_encode(E, st);
-        free(bd);
         if (rc != ZXC_OK) return rc;
         zxc_asm_tile_sums<<<n_tiles, ASM_THREADS, 0, st>>>(d_sizes, n_blocks, d_tiles);
         zxc_asm_scan_tiles<<<1, ASM_SCAN_THREADS, 0, st>>>(d_tiles, n_tiles, state, F);
@@ -1313,6 +1323,163 @@ extern "C" int zxg_compress_device(const void* d_src, uint64_t src_size, void* d
         launch_compact(d_stage, F.staging_stride, d_offs, d_sizes, d_dst8 + 16 /* file header */, n_blocks, st);
     }
     zxc_asm_finish<<<1, 1, 0, st>>>(d_dst8, state, F, (long long*)d_result);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* many device-resident buffers compressed in one call                       */
+/* (zxc_b200_compress_device_batch: kernels in zxc_cbatch.cuh)               */
+/* ------------------------------------------------------------------------- */
+/* Scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned):
+ *   CBatchState | frames (n x CBatchFrame) | first blocks (n x u64) | frame tile sums (2 per tile) | dictionary region
+ *   (with a dictionary) | offsets (nb_max x u64) | sizes (nb_max x u32) | block tile sums | room: the pool (256 x
+ *   pool_units bytes), then one encode slot
+ * Everything but the pool follows from (n, options, pool_units): nb_max = max(1, pool / (staging_stride + 256)) is the
+ * most blocks a pool can hold (every block's share, with its frame's input, is at least that).  The call takes the
+ * largest pool whose layout fits the scratch, and launches W = min(resident grid, nb_max) encode warps (whole CTAs
+ * from ENC_WARPS_PER_CTA up); those whose slot, counted down from the room's end, reaches the pool's used part exit. */
+struct CBatchLayout {
+    size_t frames, first, ftiles, dict, offs, sizes, btiles, pool, total, wstride;
+    u32 W, nb_max, stride;
+    u64 pool_units;
+};
+#define CB_FRAMES_MAX (1u << 30)
+
+static void cb_layout(u32 n, u32 bs, int level, u32 dict_size, u64 pool_units, CBatchLayout* L) {
+    const size_t n_tiles = ((size_t)n + ASM_TILE - 1) / ASM_TILE;
+    L->stride = enc_staging_stride(bs);
+    L->wstride = enc_layout(bs, level).total;
+    const u64 nb = pool_units * 256 / ((u64)L->stride + 256);
+    L->nb_max = nb ? (u32)nb : 1u;
+    const u32 resident = (u32)(g_sm_count > 0 ? g_sm_count : 132) * ENC_CTAS_PER_SM * ENC_WARPS_PER_CTA;
+    u32 W = L->nb_max < resident ? L->nb_max : resident;
+    if (W >= ENC_WARPS_PER_CTA) W -= W % ENC_WARPS_PER_CTA;
+    L->W = W;
+    L->pool_units = pool_units;
+    size_t o = CB_STATE_BYTES;
+    L->frames = o;
+    o += r256((size_t)n * sizeof(CBatchFrame));
+    L->first = o;
+    o += r256((size_t)n * 8);
+    L->ftiles = o;
+    o += r256(n_tiles * 16);
+    L->dict = o;
+    if (dict_size) o += r256(enc_dict_bytes(dict_size));
+    L->offs = o;
+    o += r256((size_t)L->nb_max * 8);
+    L->sizes = o;
+    o += r256((size_t)L->nb_max * 4);
+    L->btiles = o;
+    o += r256(((size_t)L->nb_max + ASM_TILE - 1) / ASM_TILE * 8);
+    L->pool = o;
+    o += (size_t)pool_units * 256 + L->wstride;
+    L->total = o + 256; /* base alignment slack */
+}
+
+extern "C" size_t zxg_compress_batch_scratch_bytes(uint32_t max_frames, uint64_t max_total_src, uint32_t block_size,
+                                                   int level, uint32_t dict_size) {
+    if (zxg_init() != ZXC_OK || max_frames > CB_FRAMES_MAX || max_total_src > (1ull << 50)) return 0;
+    /* the most any batch of max_frames frames of max_total_src bytes can take: input copies of r256(size + 64) bytes
+     * and ceil(size / block_size) staging slots for each of at most m non-empty ones */
+    const u64 m = max_frames < max_total_src ? max_frames : max_total_src;
+    const u64 in = (max_total_src + 319ull * m) / 256;
+    const u64 blocks = (max_total_src + m * (block_size - 1)) / block_size;
+    const u64 need = in + blocks * (enc_staging_stride(block_size) / 256);
+    if (need > CB_POOL_UNITS_MAX) return 0;
+    /* and room for the encode slots of the warps that pool launches, beyond the one the layout always has */
+    CBatchLayout L;
+    cb_layout(max_frames, block_size, level, dict_size, need, &L);
+    const u64 pool = need + (u64)(L.W - 1) * (L.wstride / 256);
+    if (pool > CB_POOL_UNITS_MAX) return 0;
+    cb_layout(max_frames, block_size, level, dict_size, pool, &L);
+    return L.total;
+}
+
+extern "C" int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, uint32_t block_size,
+                                         int level, int checksum, int seekable, const void* h_dict,
+                                         uint32_t dict_size, const uint8_t* h_dict_huf_lens, const uint8_t* header,
+                                         const uint8_t* eof, void* d_scratch, size_t scratch_size, int64_t* d_results,
+                                         void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    const u32 n = n_frames;
+    if (n > CB_FRAMES_MAX) return ZXC_ERROR_MEMORY;
+    const u32 dsz = h_dict && dict_size ? dict_size : 0;
+    CBatchLayout L;
+    cb_layout(n, block_size, level, dsz, 0, &L);
+    if (L.total > scratch_size) return ZXC_ERROR_MEMORY;
+    u64 lo = 0, hi = CB_POOL_UNITS_MAX; /* the largest pool whose layout fits */
+    while (lo < hi) {
+        const u64 mid = lo + (hi - lo + 1) / 2;
+        cb_layout(n, block_size, level, dsz, mid, &L);
+        if (L.total <= scratch_size) lo = mid;
+        else hi = mid - 1;
+    }
+    cb_layout(n, block_size, level, dsz, lo, &L);
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    CBatchArgs A;
+    A.frames = d_frames;
+    A.results = (long long*)d_results;
+    A.st = (CBatchState*)base;
+    A.F = (CBatchFrame*)(base + L.frames);
+    A.first = (unsigned long long*)(base + L.first);
+    A.ftiles = (unsigned long long*)(base + L.ftiles);
+    A.btiles = (unsigned long long*)(base + L.btiles);
+    A.offs = (unsigned long long*)(base + L.offs);
+    A.sizes = (u32*)(base + L.sizes);
+    A.staging = base + L.pool;
+    A.pool_units = L.pool_units;
+    A.wstride = L.wstride;
+    A.n = n;
+    A.nb_max = L.nb_max;
+    A.warps = L.W;
+    A.block_size = block_size;
+    A.staging_stride = L.stride;
+    A.checksum = checksum ? 1u : 0u;
+    A.seekable = seekable ? 1u : 0u;
+    memcpy(A.header, header, 16);
+    memcpy(A.eof, eof, 8);
+    EncodeParams P;
+    memset(&P, 0, sizeof P);
+    P.staging = A.staging;
+    P.out_size = A.sizes;
+    /* the W encode slots end at the room's end: slot g at scratch + g * wstride; those below the room never run */
+    P.scratch = A.staging + (size_t)L.pool_units * 256 + L.wstride - (size_t)L.W * L.wstride;
+    P.counter = &A.st->counter;
+    if (dsz) {
+        const int rc = enc_stage_dict(P, base + L.dict, h_dict, dsz, level, h_dict_huf_lens, st);
+        if (rc != ZXC_OK) return rc;
+    }
+    P.scratch_stride = L.wstride;
+    P.block_size = block_size;
+    P.staging_stride = L.stride;
+    P.level = (u32)level;
+    P.checksum = A.checksum;
+    P.dict_size = dsz;
+    const u32 sms = (u32)(g_sm_count > 0 ? g_sm_count : 132);
+    const u32 n_tiles = (n + ASM_TILE - 1) / ASM_TILE;
+    const u32 per_frame = (n + CB_THREADS - 1) / CB_THREADS;
+    const u32 b_tiles = (L.nb_max + ASM_TILE - 1) / ASM_TILE;
+    const u32 by_warp = (L.nb_max + CB_THREADS / 32 - 1) / (CB_THREADS / 32);
+    const u32 by_thread = (L.nb_max + CB_THREADS - 1) / CB_THREADS;
+    zxc_cbatch_tiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_cbatch_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_cbatch_place<<<per_frame, CB_THREADS, 0, st>>>(A);
+    zxc_cbatch_gather<<<by_warp < sms * 16 ? by_warp : sms * 16, CB_THREADS, 0, st>>>(A);
+    const u32 grid = L.W >= ENC_WARPS_PER_CTA ? L.W / ENC_WARPS_PER_CTA : 1u;
+    const u32 threads = L.W >= ENC_WARPS_PER_CTA ? ENC_CTA_THREADS : 32u * L.W;
+    if (level >= 6) zxc_encode_batch_kernel<true><<<grid, threads, 0, st>>>(P, A);
+    else zxc_encode_batch_kernel<false><<<grid, threads, 0, st>>>(P, A);
+    zxc_cbatch_sums<<<b_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_cbatch_bscan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_cbatch_offsets<<<b_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_cbatch_fit<<<per_frame, CB_THREADS, 0, st>>>(A);
+    zxc_cbatch_blocks<<<by_thread < sms * 16 ? by_thread : sms * 16, CB_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 10, __ATOMIC_RELAXED);
+    launch_compact(A.staging, L.stride, A.offs, A.sizes, NULL /* absolute destinations */, L.nb_max, st);
+    zxc_cbatch_finish<<<per_frame, CB_THREADS, 0, st>>>(A);
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }

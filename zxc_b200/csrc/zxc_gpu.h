@@ -92,6 +92,17 @@ int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_fra
                                 int checksum_enabled, void* d_scratch, size_t scratch_size, int64_t* d_results,
                                 void* stream);
 
+/* Many device-resident buffers compressed in one call (zxc_b200_compress_device_batch; kernels in zxc_cbatch.cuh), with
+ * the options checked and the shared frame bytes (file header, EOF block header) written by the host.  Scratch for up
+ * to max_frames buffers of at most max_total_src bytes in all (0 without a device or when that cannot be planned);
+ * ZXC_ERROR_MEMORY when the scratch holds less than that for empty buffers. */
+size_t zxg_compress_batch_scratch_bytes(uint32_t max_frames, uint64_t max_total_src, uint32_t block_size, int level,
+                                        uint32_t dict_size);
+int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, uint32_t block_size, int level,
+                              int checksum, int seekable, const void* h_dict, uint32_t dict_size,
+                              const uint8_t* h_dict_huf_lens, const uint8_t* header, const uint8_t* eof,
+                              void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);
+
 /* Device-resident seekable frames (zxc_dseek.c; kernels in zxc_dseek.cuh).  What a range call needs of its handle. */
 typedef struct {
     const void* d_src;

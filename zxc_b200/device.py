@@ -5,7 +5,8 @@ through the host.  ``decompress`` decodes such a frame with zxc_b200_decode_bloc
 compress call emitted.  ``decompress_frame`` decodes any frame held in a uint8 CUDA tensor with
 zxc_b200_decompress_device, which plans, decodes and checks it on the device.  ``SeekableFrame`` decodes byte ranges of
 a seekable frame in HBM with zxc_b200_seekable_device_decompress_ranges.  ``decompress_frames`` decodes many frames
-in one zxc_b200_decompress_device_batch call.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
+in one zxc_b200_decompress_device_batch call, and ``compress_frames`` compresses many tensors into one frame each in
+one zxc_b200_compress_device_batch call.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
 """
 import ctypes as C
 from dataclasses import dataclass
@@ -322,6 +323,77 @@ def decompress_frames(frames, capacities=None, *, out=None, dict=None, dict_huf=
                                                       scratch_size, results.data_ptr(), stream.cuda_stream)
             if rc != 0:
                 raise ZxcError(rc, "zxc_b200_decompress_device_batch")
+    return out, results
+
+
+lib.zxc_b200_compress_device_batch_scratch_size.restype = C.c_size_t
+lib.zxc_b200_compress_device_batch_scratch_size.argtypes = [C.c_uint32, C.c_uint64, C.c_void_p]
+lib.zxc_b200_compress_device_batch.restype = C.c_int
+lib.zxc_b200_compress_device_batch.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p,
+                                               C.c_void_p]
+
+
+def compress_frames(srcs, *, level=0, block_size=0, checksum=False, seekable=False, dict=None, dict_huf=None, out=None,
+                    stream=None):
+    """Compress many contiguous CUDA tensors (their bytes), all on one device, into one ZXC frame each in one batch call.
+
+    Returns (outs, results): outs[i] is the tensor frame i was written to (by default zxc_compress_bound(len) bytes),
+    results an int64 CUDA tensor where results[i] is exactly what compress's zxc_b200_compress_device call gives
+    input i alone: its frame size (the frame is outs[i][:results[i]]) or a negative zxc_error_t code.  `out`, a list of
+    contiguous uint8 tensors on the inputs' device, one per input, takes the frames instead.  The work runs on `stream`
+    (default: the current stream), which first waits for the current stream; nothing synchronises.  Argument errors
+    raise ValueError before anything is enqueued; a rejected call raises ZxcError with its code.  dict / dict_huf are
+    host bytes, one dictionary for the batch."""
+    srcs = list(srcs)
+    if not srcs:
+        raise ValueError("srcs is empty")
+    dev = srcs[0].device
+    for t in srcs:
+        if not t.is_cuda or not t.is_contiguous():
+            raise ValueError("every input must be a contiguous CUDA tensor")
+        if t.device != dev:
+            raise ValueError(f"every input must be on {dev}, not {t.device}")
+    srcs = [t.reshape(-1).view(torch.uint8) for t in srcs]
+    n = len(srcs)
+    if out is not None:
+        out = list(out)
+        if len(out) != n:
+            raise ValueError("out must hold one tensor per input")
+        for o in out:
+            _check_out(o, dev)
+    o = _Opts(level=level, block_size=block_size, checksum_enabled=int(bool(checksum)), seekable=int(bool(seekable)))
+    keep = []
+    if dict is not None:
+        d = bytes(dict)
+        keep.append(d)
+        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+        if dict_huf is not None:
+            h = bytes(dict_huf)
+            keep.append(h)
+            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    # 0 for options the call rejects (it then gives their exact code below with a token scratch), or a batch too large
+    scratch_size = int(lib.zxc_b200_compress_device_batch_scratch_size(n, sum(t.numel() for t in srcs), C.byref(o)))
+    with torch.cuda.device(dev):
+        current = torch.cuda.current_stream(dev)
+        stream = stream or current
+        if stream != current:
+            # the inputs were made (or written) on the current stream; the caller may drop them on return
+            stream.wait_stream(current)
+            for t in srcs + (out or []):
+                t.record_stream(stream)
+        with torch.cuda.stream(stream):
+            if out is None:
+                out = [torch.empty(int(lib.zxc_compress_bound(t.numel())), dtype=torch.uint8, device=dev) for t in srcs]
+            # page-locked, so the upload does not wait for the stream (the host allocator keeps it until it ran)
+            desc = torch.tensor([[t.data_ptr() if t.numel() else 0, t.numel(), d.data_ptr() if d.numel() else 0,
+                                  d.numel()] for t, d in zip(srcs, out)], dtype=torch.int64)
+            desc = desc.pin_memory().to(dev, non_blocking=True)
+            scratch = torch.empty(max(scratch_size, 1), dtype=torch.uint8, device=dev)
+            results = torch.empty(n, dtype=torch.int64, device=dev)
+            rc = lib.zxc_b200_compress_device_batch(desc.data_ptr(), n, C.byref(o), scratch.data_ptr(), scratch_size,
+                                                    results.data_ptr(), stream.cuda_stream)
+            if rc != 0:
+                raise ZxcError(rc, "zxc_b200_compress_device_batch")
     return out, results
 
 
