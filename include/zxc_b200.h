@@ -152,7 +152,7 @@ ZXC_EXPORT size_t zxc_b200_decompress_device_scratch_size(uint64_t dst_capacity,
  * past a run.  In a frame that ends with its EOF block and footer every run lies at least 20 bytes before the end,
  * so those loads stay inside d_src[0 .. src_size).  Only a truncated frame, whose last block runs to src_size, may
  * have up to 8 bytes behind d_src + src_size read: keep 8 readable bytes there when frames come from an untrusted
- * source.  d_src and d_dst must not overlap (in-place decode is zxc_decompress_inplace).  Without a dictionary the call makes no host synchronisation and no allocation and may be
+ * source.  d_src and d_dst must not overlap (in-place decode is zxc_b200_decompress_inplace_device).  Without a dictionary the call makes no host synchronisation and no allocation and may be
  * captured in a CUDA graph.  Kernel launches per call (zxc_b200_launch_count): 12 + k * (2 + c), where k is the
  * number of block sizes from 4 KiB up to B (B = 64 KiB: k = 5) and c = 1 when opts->checksum_enabled, else 0.  The
  * frame is planned on the device (a parallel plan from its SEK table when it has one, else a sequential walk of its
@@ -161,6 +161,72 @@ ZXC_EXPORT size_t zxc_b200_decompress_device_scratch_size(uint64_t dst_capacity,
 ZXC_EXPORT int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
                                           const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
                                           int64_t* d_result, void* stream);
+
+/* ---- in-place decode in HBM: the device twin of zxc_decompress_inplace ---- */
+/* Device scratch for zxc_b200_decompress_inplace_device with buffers of at most buffer_capacity bytes, frames whose
+ * header block size is at most block_size, and a staging window of `window` compressed bytes per round (0: bad block
+ * size, no device, or a capacity too large to plan).  It is zxc_b200_decompress_device_scratch_size(buffer_capacity,
+ * block_size), plus two round tables of 28 x min(J, window / 8 + 1) bytes, 8 bytes per smallest window of the buffer
+ * and a staging area of window + block_size + 76 bytes (rounded up to 256-byte regions).  Windows are whole multiples
+ * of 4 KiB: `window` is rounded up to one, raised to the smallest window W_min = 4 x block_size + 4096, and lowered to
+ * buffer_capacity rounded up to 4 KiB, which decodes any frame in the buffer in one round. */
+ZXC_EXPORT size_t zxc_b200_decompress_inplace_device_scratch_size(uint64_t buffer_capacity, uint32_t block_size,
+                                                                 uint64_t window);
+
+/* zxc_decompress_inplace_bound for a frame in device memory, d_src[0 .. src_size): reads its 16 header bytes and its
+ * footer with two copies on `stream`, which it synchronises.  0 where zxc_decompress_inplace_bound gives 0, and
+ * without a device. */
+ZXC_EXPORT size_t zxc_b200_decompress_inplace_device_bound(const void* d_src, uint64_t src_size, void* stream);
+
+/* Decodes the frame of comp_size bytes that lies flush-right in d_buffer[0 .. buffer_capacity) (device memory) into
+ * d_buffer[0 ..), on `stream`, asynchronously, with no second buffer: the device memory it takes is the buffer and
+ * the scratch, against frame + output + scratch for zxc_b200_decompress_device.
+ * *d_result (one device int64) and d_buffer[0 .. *d_result) when it is not negative become exactly what this
+ * library's zxc_decompress_inplace returns and writes for the same buffer contents, buffer_capacity, comp_size and
+ * opts, but for the two limits below; frames the reference's encoder writes never reach them.  (The reference's
+ * zxc_decompress_inplace also rejects buffer_capacity - comp_size < block_size + 2112; neither call does.)
+ *   opts       as for zxc_b200_decompress_device: checksum_enabled, and a dictionary in HOST memory, staged the same
+ *              way (a host copy: the call then may wait for the stream and cannot be captured in a CUDA graph)
+ *   d_scratch  zxc_b200_decompress_inplace_device_scratch_size(buffer_capacity, b, window) bytes; the call finds the
+ *              block size B and the window W from scratch_size and buffer_capacity alone: B is the largest block size
+ *              whose layout with the smallest window fits, and W the largest window (a multiple of 4 KiB, up to
+ *              buffer_capacity rounded up to 4 KiB) that then fits.  Frames with blocks larger than B get ZXC_ERROR_MEMORY in *d_result, as from
+ *              zxc_b200_decompress_device.  A scratch sized for (b, window) gives B = b and W = window unless the
+ *              window is larger than the growth of the decode kernels' per-warp scratch from b to 2b, about 2.7 x b
+ *              per warp for one warp per 4 KiB of buffer_capacity, up to the resident grid (4 224 warps on an H100):
+ *              never for buffers below about 17 MiB, else above about 47 MiB at 4 KiB blocks and 730 MiB at 64 KiB.
+ *              Such a window gives a larger B and a smaller W: the same result, in more rounds.
+ * Returns ZXC_OK once enqueued, or what the host decides without reading the buffer, in this order:
+ * ZXC_ERROR_NULL_INPUT (a NULL d_buffer, comp_size below file header + footer or above buffer_capacity, as
+ * zxc_decompress_inplace; also a NULL d_scratch or d_result), ZXC_ERROR_DICT_TOO_LARGE, ZXC_B200_ERROR_NO_DEVICE, then
+ * ZXC_ERROR_MEMORY when the scratch is below zxc_b200_decompress_inplace_device_scratch_size(buffer_capacity, 4096, 0).
+ * The device writes the rest to *d_result, in zxc_decompress_inplace's order: its own checks first (BAD_MAGIC,
+ * BAD_HEADER for any file-header reject, CORRUPT_DATA for a footer size the frame cannot hold, DST_TOO_SMALL when
+ * buffer_capacity is below the decoded size plus zxc_decompress_inplace_bound's margin), then everything
+ * zxc_b200_decompress_device decides for d_src = d_buffer + buffer_capacity - comp_size, d_dst = d_buffer and
+ * dst_capacity = buffer_capacity, with that call's limits.  Two limits of this call give ZXC_ERROR_MEMORY as well:
+ *   (a) the round schedule cannot decode the frame without overwriting compressed bytes a later round still has to
+ *       stage, or a block is longer on disk than B + 12 bytes (the largest block the reference's encoder writes) and
+ *       would not fit its round's staged copy.  This is decided after the plan and before the first byte of the buffer
+ *       is written: the buffer is then unchanged.  Only a frame with more than one round can reach it;
+ *   (b) the frame needs zxc_b200_decompress_device's general re-plan (non-final blocks that decode to less than the
+ *       block size) and the call runs more than one round.
+ * With one round (W >= comp_size) neither applies.  On any other negative result the buffer's contents are
+ * unspecified: the decode is in place, so the frame is consumed.
+ * How it works (DESIGN.md section 7j): the frame is planned where it lies; then, in R = ceil(comp_size / W) rounds,
+ * round k copies frame bytes [k W - 8, min((k + 1) W + B + 20, comp_size)) into the scratch and decodes the blocks
+ * whose headers lie in [k W, (k + 1) W) from that copy into the buffer.
+ * Nothing outside d_buffer[0 .. buffer_capacity), the scratch and *d_result is written, and nothing outside
+ * d_buffer[0 .. buffer_capacity) is read: the decode kernels read the staged copy, so their read-past stays inside
+ * the scratch; d_buffer may have any alignment.  Without a dictionary there is no host synchronisation and no
+ * allocation, and the call may be captured in a CUDA graph; a replay consumes the frame, so restore the buffer before
+ * each one.  Kernel launches per call (zxc_b200_launch_count): 16 + R * (1 + k * (2 + c)), k and c as for
+ * zxc_b200_decompress_device with the B above (plan: 6, the in-place probe and the round plan: 2; per round one table
+ * kernel and the decode kernels; the last round's gather, check, decide, the re-plan limit: 4; the general split: 4);
+ * R and k follow from (comp_size, buffer_capacity, scratch_size).  Each round also makes one device-to-device copy. */
+ZXC_EXPORT int zxc_b200_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,
+                                                  const zxc_decompress_opts_t* opts, void* d_scratch,
+                                                  size_t scratch_size, int64_t* d_result, void* stream);
 
 /* ---- many device-resident frames in one call: zxc_b200_decompress_device over a batch ---- */
 /* one frame of a batch; the array of them lives in DEVICE memory */

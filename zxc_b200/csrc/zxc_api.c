@@ -726,24 +726,29 @@ static uint64_t inplace_margin(uint64_t dsize, size_t bs, int has_cs) {
            (ZXF_BLOCK_HDR + nb * ZXF_SEEK_ENTRY) + ZXC_FILE_FOOTER_SIZE + ZXF_TAIL_PAD;
 }
 
-static int inplace_probe(const uint8_t* comp, size_t comp_size, uint64_t* dsize, uint64_t* margin) {
-    if (zxf_le32(comp) != ZXF_MAGIC) return ZXC_ERROR_BAD_MAGIC;
+/* on the frame's 16 header bytes and its footer's 8-byte size */
+static int inplace_probe(const uint8_t* header, uint64_t d, size_t comp_size, uint64_t* dsize, uint64_t* margin) {
+    if (zxf_le32(header) != ZXF_MAGIC) return ZXC_ERROR_BAD_MAGIC;
     zxf_file_header_t fh;
-    if (zxf_read_file_header(comp, comp_size, &fh, 1) != ZXC_OK) return ZXC_ERROR_BAD_HEADER;
-    const uint64_t d = zxf_le64(comp + comp_size - ZXC_FILE_FOOTER_SIZE);
+    if (zxf_read_file_header(header, ZXC_FILE_HEADER_SIZE, &fh, 1) != ZXC_OK) return ZXC_ERROR_BAD_HEADER;
     if (!zxf_dsize_plausible(d, fh.block_size, comp_size)) return ZXC_ERROR_CORRUPT_DATA;
     *dsize = d;
     *margin = inplace_margin(d, fh.block_size, fh.has_checksum);
     return ZXC_OK;
 }
 
-size_t zxc_decompress_inplace_bound(const void* src, const size_t src_size) {
-    if (!src || src_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE) return 0;
-    uint64_t d = 0, m = 0;
-    if (inplace_probe((const uint8_t*)src, src_size, &d, &m) != ZXC_OK) return 0;
+static size_t inplace_bound(const uint8_t* header, uint64_t d, size_t src_size) {
+    uint64_t m = 0;
+    if (inplace_probe(header, d, src_size, &d, &m) != ZXC_OK) return 0;
     const uint64_t by_payload = d + m;
     const uint64_t by_placement = (uint64_t)src_size + m;
     return (size_t)(by_payload > by_placement ? by_payload : by_placement);
+}
+
+size_t zxc_decompress_inplace_bound(const void* src, const size_t src_size) {
+    if (!src || src_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE) return 0;
+    const uint8_t* s = (const uint8_t*)src;
+    return inplace_bound(s, zxf_le64(s + src_size - ZXC_FILE_FOOTER_SIZE), src_size);
 }
 
 int64_t zxc_decompress_inplace(void* buffer, const size_t buffer_capacity, const size_t comp_size,
@@ -753,7 +758,7 @@ int64_t zxc_decompress_inplace(void* buffer, const size_t buffer_capacity, const
     uint8_t* buf = (uint8_t*)buffer;
     const uint8_t* comp = buf + (buffer_capacity - comp_size);
     uint64_t d = 0, m = 0;
-    const int rc = inplace_probe(comp, comp_size, &d, &m);
+    const int rc = inplace_probe(comp, zxf_le64(comp + comp_size - ZXC_FILE_FOOTER_SIZE), comp_size, &d, &m);
     if (rc != ZXC_OK) return rc;
     if (d > buffer_capacity || buffer_capacity - d < m) return ZXC_ERROR_DST_TOO_SMALL;
     /* source and destination overlap: decompress_frame then takes the in-HBM route, where the whole
@@ -1028,6 +1033,41 @@ int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst
     return zxg_decompress_device(d_src, src_size, d_dst, dst_capacity, dict_size ? dict : NULL, (uint32_t)dict_size,
                                  arc == 1 ? dict_huf : NULL, did, arc, opts ? opts->checksum_enabled : 0, d_scratch,
                                  scratch_size, d_result, stream);
+}
+
+size_t zxc_b200_decompress_inplace_device_scratch_size(uint64_t buffer_capacity, uint32_t block_size, uint64_t window) {
+    if (!zxf_valid_block_size(block_size)) return 0;
+    return zxg_decompress_inplace_scratch_bytes(buffer_capacity, block_size, window);
+}
+
+size_t zxc_b200_decompress_inplace_device_bound(const void* d_src, uint64_t src_size, void* stream) {
+    if (!d_src || src_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE || zxg_init() != ZXC_OK) return 0;
+    uint8_t header[ZXC_FILE_HEADER_SIZE], footer[8];
+    if (zxg_d2h_sync(header, d_src, sizeof header, stream) != ZXC_OK ||
+        zxg_d2h_sync(footer, (const uint8_t*)d_src + src_size - ZXC_FILE_FOOTER_SIZE, sizeof footer, stream) != ZXC_OK)
+        return 0;
+    return inplace_bound(header, zxf_le64(footer), src_size);
+}
+
+/* The host decides what zxc_decompress_inplace decides without the frame's bytes, then what
+ * zxc_b200_decompress_device decides without them; the device decides the rest (zxc_dinplace.cuh). */
+int zxc_b200_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,
+                                       const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                                       int64_t* d_result, void* stream) {
+    if (!d_buffer || comp_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE || comp_size > buffer_capacity ||
+        !d_scratch || !d_result)
+        return ZXC_ERROR_NULL_INPUT;
+    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
+    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
+    const int arc = dict_size ? dict_huf_attach(dict_huf) : 0;
+    return zxg_decompress_inplace_device(d_buffer, buffer_capacity, comp_size, dict_size ? dict : NULL,
+                                         (uint32_t)dict_size, arc == 1 ? dict_huf : NULL, did, arc,
+                                         opts ? opts->checksum_enabled : 0, d_scratch, scratch_size, d_result, stream);
 }
 
 size_t zxc_b200_decompress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_capacity,

@@ -28,6 +28,7 @@
 #include "zxc_dbatch.cuh"
 #include "zxc_cbatch.cuh"
 #include "zxc_dplan.cuh"
+#include "zxc_dinplace.cuh"
 #include "zxc_dseek.cuh"
 #include "zxc_train.cuh"
 
@@ -1494,6 +1495,27 @@ extern "C" int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint3
  * J = ceil(dst_capacity / ZXC_BLOCK_SIZE_MIN) + 2: every block but the last of a frame the reference's encoder
  * writes holds block_size >= ZXC_BLOCK_SIZE_MIN bytes, so such a frame fits the table when its output fits
  * dst_capacity. */
+/* A decode's dictionary and its literal table (when given) into the scratch's dictionary region at d_region, through
+ * a pageable host copy: the caller's dictionary has been read when the call returns, whatever memory it is in
+ * (host_bounce).  Both device pointers stay NULL without a dictionary. */
+static int dec_stage_dict(u8* d_region, const void* h_dict, u32 dict_size, const void* h_dict_huf, cudaStream_t st,
+                          u8** d_dict, u8** d_huf) {
+    *d_dict = NULL;
+    *d_huf = NULL;
+    if (!h_dict || !dict_size) return ZXC_OK;
+    *d_dict = d_region;
+    const size_t dbytes = (size_t)dict_size + (h_dict_huf ? ZXC_HUF_TABLE_SIZE : 0);
+    u8* b = (u8*)host_bounce(h_dict, dict_size, dbytes);
+    if (!b) return ZXC_ERROR_MEMORY;
+    if (h_dict_huf) {
+        memcpy(b + dict_size, h_dict_huf, ZXC_HUF_TABLE_SIZE);
+        *d_huf = d_region + dict_size;
+    }
+    const cudaError_t e = cudaMemcpyAsync(d_region, b, dbytes, cudaMemcpyHostToDevice, st);
+    free(b);
+    return e == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
 struct DevDecLayout {
     size_t dict, plan, jobs, status, sizes, tiles, slots, dec, dec_bytes, total;
     u32 J, probe_warps, room;
@@ -1543,6 +1565,96 @@ static void launch_dsplit(const DSplitArgs& D, u32 phase, u32 grid, cudaStream_t
     zxc_dsplit_decode<HAS_DICT><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(D, phase);
 }
 
+/* the general split's four launches (zxc_dplan.cuh); they exit at once unless zxc_dplan_decide asked for it */
+static void launch_dsplit_all(const DSplitArgs& D, bool has_dict, cudaStream_t st) {
+    const u32 probe_grid = (D.probe_warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
+    const u32 dec_grid = (u32)grid_for(D.a.J);
+    if (has_dict) launch_dsplit<true>(D, 0, probe_grid, st);
+    else launch_dsplit<false>(D, 0, probe_grid, st);
+    zxc_dsplit_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(D.a);
+    if (has_dict) launch_dsplit<true>(D, 1, dec_grid, st);
+    else launch_dsplit<false>(D, 1, dec_grid, st);
+    zxc_dsplit_final<<<1, ASM_SCAN_THREADS, 0, st>>>(D.a);
+    __atomic_add_fetch(&g_launches, 4, __ATOMIC_RELAXED);
+}
+
+/* zxc_dplan.cuh's arguments over a DevDecLayout at base */
+static DPlanArgs dplan_args(u8* base, const DevDecLayout& L, const void* d_src, uint64_t src_size,
+                            uint64_t dst_capacity, u32 bs, bool has_dict, uint32_t dict_id, int huf_verdict,
+                            int checksum_enabled, int64_t* d_result) {
+    DPlanArgs A;
+    A.src = (const u8*)d_src;
+    A.src_size = src_size;
+    A.dst_capacity = dst_capacity;
+    A.plan = (zxc_b200_job_t*)(base + L.plan);
+    A.jobs = (zxc_b200_job_t*)(base + L.jobs);
+    A.status = (i32*)(base + L.status);
+    A.sizes = (i32*)(base + L.sizes);
+    A.tiles = (unsigned long long*)(base + L.tiles);
+    A.st = (DPlanState*)base;
+    A.result = (long long*)d_result;
+    A.J = L.J;
+    A.max_block_size = bs;
+    A.dict_id = dict_id;
+    A.have_dict = has_dict ? 1u : 0u;
+    A.huf_verdict = huf_verdict;
+    A.checksum_enabled = checksum_enabled ? 1u : 0u;
+    return A;
+}
+
+/* the frame's plan: probe, SEK-guided plan, walk, and the job table */
+static void launch_dplan(const DPlanArgs& A, cudaStream_t st) {
+    const u32 n_tiles = (A.J + ASM_TILE - 1) / ASM_TILE;
+    const u32 per_job = (A.J + DP_THREADS - 1) / DP_THREADS;
+    zxc_dplan_probe<<<1, 1, 0, st>>>(A);
+    zxc_dplan_sek_tiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dplan_sek_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_dplan_sek_blocks<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dplan_walk<<<1, 32, 0, st>>>(A);
+    zxc_dplan_place<<<per_job, DP_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
+}
+
+/* one launch_decode per slot: block sizes up to bs, checksum verification off / on; only the frame's has work.  The
+ * job table has J entries and the counters were preset on the device. */
+static int launch_dplan_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* jobs, i32* status, u32 J,
+                               DPlanState* S, const u8* d_dict, u32 dict_size, const u8* d_huf, u8* dec,
+                               size_t dec_bytes, u32 bs, int checksum_enabled, cudaStream_t st) {
+    for (u32 b = ZXC_BLOCK_SIZE_MIN; b <= bs; b <<= 1) {
+        const u32 lg = (u32)__builtin_ctz(b) - ZXC_BLOCK_SIZE_MIN_LOG2;
+        for (int v = 0; v <= (checksum_enabled ? 1 : 0); v++) {
+            const int rc = launch_decode(d_src, d_dst, jobs, J, status, d_dict, dict_size, d_huf, dec, dec_bytes, b,
+                                         v, S->ctr[lg * 2 + v], st, 1);
+            if (rc != ZXC_OK) return rc;
+        }
+    }
+    return ZXC_OK;
+}
+
+/* the general split's arguments over a DevDecLayout at base */
+static DSplitArgs dsplit_args(const DPlanArgs& A, u8* base, const DevDecLayout& L, void* d_dst, u8* d_dict,
+                              u8* d_huf, u32 dict_size, u32 bs) {
+    DSplitArgs D;
+    D.a = A;
+    D.dst = (u8*)d_dst;
+    D.slots = base + L.slots;
+    D.scratch = base + L.dec;
+    D.dict = d_dict;
+    D.dict_huf = d_huf;
+    D.dict_size = d_dict ? dict_size : 0;
+    D.scratch_stride = scratch_stride_for(bs);
+    D.room = L.room;
+    D.probe_warps = L.probe_warps;
+    return D;
+}
+
+/* the first failing job, then zxc_decompress's verdict or the general split's go-ahead */
+static void launch_dplan_verdict(const DPlanArgs& A, cudaStream_t st) {
+    zxc_dplan_check<<<(A.J + DP_THREADS - 1) / DP_THREADS, DP_THREADS, 0, st>>>(A);
+    zxc_dplan_decide<<<1, 1, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 2, __ATOMIC_RELAXED);
+}
+
 extern "C" int zxg_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
                                      const void* h_dict, uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id,
                                      int huf_verdict, int checksum_enabled, void* d_scratch, size_t scratch_size,
@@ -1561,81 +1673,160 @@ extern "C" int zxg_decompress_device(const void* d_src, uint64_t src_size, void*
     if (!bs) return ZXC_ERROR_MEMORY;
     cudaStream_t st = (cudaStream_t)stream;
     u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
-    DPlanState* S = (DPlanState*)base;
     const bool has_dict = h_dict && dict_size;
-    u8* d_dict = NULL;
-    u8* d_huf = NULL;
-    if (has_dict) { /* read before the call returns, whatever memory the caller's dictionary is in (host_bounce) */
-        d_dict = base + L.dict;
-        const size_t dbytes = (size_t)dict_size + (h_dict_huf ? ZXC_HUF_TABLE_SIZE : 0);
-        u8* b = (u8*)host_bounce(h_dict, dict_size, dbytes);
-        if (!b) return ZXC_ERROR_MEMORY;
-        if (h_dict_huf) {
-            memcpy(b + dict_size, h_dict_huf, ZXC_HUF_TABLE_SIZE);
-            d_huf = d_dict + dict_size;
-        }
-        const cudaError_t e = cudaMemcpyAsync(d_dict, b, dbytes, cudaMemcpyHostToDevice, st);
-        free(b);
-        if (e != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    u8 *d_dict, *d_huf;
+    const int drc = dec_stage_dict(base + L.dict, h_dict, dict_size, h_dict_huf, st, &d_dict, &d_huf);
+    if (drc != ZXC_OK) return drc;
+    const DPlanArgs A = dplan_args(base, L, d_src, src_size, dst_capacity, bs, has_dict, dict_id, huf_verdict,
+                                   checksum_enabled, d_result);
+    launch_dplan(A, st);
+    const int rc = launch_dplan_decode(d_src, d_dst, A.jobs, A.status, L.J, A.st, d_dict, dict_size, d_huf,
+                                       base + L.dec, L.dec_bytes, bs, checksum_enabled, st);
+    if (rc != ZXC_OK) return rc;
+    launch_dplan_verdict(A, st);
+    launch_dsplit_all(dsplit_args(A, base, L, d_dst, d_dict, d_huf, dict_size, bs), has_dict, st);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* in-place decode of a device-resident frame (zxc_b200_decompress_inplace_  */
+/* device: kernels in zxc_dinplace.cuh)                                      */
+/* ------------------------------------------------------------------------- */
+/* Scratch layout: zxc_b200_decompress_device's (DevDecLayout for buffer_capacity and B), then, every region
+ * 256-aligned: the hazard flag | round starts (R_max + 1 x u64) | two round tables (Jr jobs) | their status arrays
+ * (Jr x i32) | the staging area of W + O + 64 bytes.  O = B + 12 (a RAW block with its checksum: the largest block the
+ * reference's encoder writes at block size B), Jr = min(J, W / 8 + 1), R_max = ceil(buffer_capacity / W_min) + 1 with
+ * W_min the smallest window. */
+struct InplaceLayout {
+    DevDecLayout d;
+    size_t hazard, rstart, rjobs[2], rstatus[2], staging, total;
+    u64 W, O;
+    u32 bs, Jr;
+};
+/* windows are whole multiples of IP_WINDOW_UNIT, from W_min = 2 (B + O) rounded up to the unit, to the buffer's
+ * capacity rounded up to it; a scratch sized for a window then gives exactly that window (unless a larger B fits) */
+#define IP_WINDOW_UNIT 4096ull
+static u64 ip_round_up(u64 v) { return (v + IP_WINDOW_UNIT - 1) / IP_WINDOW_UNIT * IP_WINDOW_UNIT; }
+static u64 ip_window_min(u32 bs) { return ip_round_up(2ull * (bs + (u64)bs + ZXF_BLOCK_HDR + ZXF_BLOCK_CKS)); }
+static u64 ip_window_max(uint64_t cap, u32 bs) {
+    const u64 w = ip_round_up(cap);
+    return w > ip_window_min(bs) ? w : ip_window_min(bs);
+}
+
+static bool ip_layout(uint64_t cap, u32 bs, u64 W, InplaceLayout* L) {
+    if (!dev_dec_layout(cap, bs, &L->d)) return false;
+    const u64 w_min = ip_window_min(bs);
+    W = W < w_min ? w_min : (W > ip_window_max(cap, bs) ? ip_window_max(cap, bs) : ip_round_up(W));
+    const u64 r_max = (cap + w_min - 1) / w_min + 1;
+    const u64 jr = W / ZXF_BLOCK_HDR + 1 < L->d.J ? W / ZXF_BLOCK_HDR + 1 : L->d.J;
+    size_t o = L->d.total - 256; /* DevDecLayout's end, before its base alignment slack */
+    L->hazard = o;
+    o += 256;
+    L->rstart = o;
+    o += r256((size_t)(r_max + 1) * 8);
+    for (int t = 0; t < 2; t++) {
+        L->rjobs[t] = o;
+        o += r256((size_t)jr * sizeof(zxc_b200_job_t));
+        L->rstatus[t] = o;
+        o += r256((size_t)jr * 4);
     }
-    DPlanArgs A;
-    A.src = (const u8*)d_src;
-    A.src_size = src_size;
-    A.dst_capacity = dst_capacity;
-    A.plan = (zxc_b200_job_t*)(base + L.plan);
-    A.jobs = (zxc_b200_job_t*)(base + L.jobs);
-    A.status = (i32*)(base + L.status);
-    A.sizes = (i32*)(base + L.sizes);
-    A.tiles = (unsigned long long*)(base + L.tiles);
-    A.st = S;
-    A.result = (long long*)d_result;
-    A.J = L.J;
-    A.max_block_size = bs;
-    A.dict_id = dict_id;
-    A.have_dict = has_dict ? 1u : 0u;
-    A.huf_verdict = huf_verdict;
-    A.checksum_enabled = checksum_enabled ? 1u : 0u;
-    const u32 n_tiles = (L.J + ASM_TILE - 1) / ASM_TILE;
-    const u32 per_job = (L.J + DP_THREADS - 1) / DP_THREADS;
-    zxc_dplan_probe<<<1, 1, 0, st>>>(A);
-    zxc_dplan_sek_tiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
-    zxc_dplan_sek_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
-    zxc_dplan_sek_blocks<<<n_tiles, ASM_THREADS, 0, st>>>(A);
-    zxc_dplan_walk<<<1, 32, 0, st>>>(A);
-    zxc_dplan_place<<<per_job, DP_THREADS, 0, st>>>(A);
-    __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
-    /* one launch slot per block size up to bs, and per checksum verification off / on; only the frame's has work */
-    u8* dec = base + L.dec;
-    for (u32 b = ZXC_BLOCK_SIZE_MIN; b <= bs; b <<= 1) {
-        const u32 lg = (u32)__builtin_ctz(b) - ZXC_BLOCK_SIZE_MIN_LOG2;
-        for (int v = 0; v <= (checksum_enabled ? 1 : 0); v++) {
-            const int rc = launch_decode(d_src, d_dst, A.jobs, L.J, A.status, d_dict, dict_size, d_huf, dec,
-                                         L.dec_bytes, b, v, S->ctr[lg * 2 + v], st, 1);
-            if (rc != ZXC_OK) return rc;
+    L->O = (u64)bs + ZXF_BLOCK_HDR + ZXF_BLOCK_CKS;
+    L->staging = o;
+    o += r256((size_t)(W + L->O + 64));
+    L->total = o + 256;
+    L->W = W;
+    L->bs = bs;
+    L->Jr = (u32)jr;
+    return true;
+}
+
+extern "C" size_t zxg_decompress_inplace_scratch_bytes(uint64_t buffer_capacity, uint32_t block_size, uint64_t window) {
+    if (zxg_init() != ZXC_OK) return 0;
+    InplaceLayout L;
+    return ip_layout(buffer_capacity, block_size, window, &L) ? L.total : 0;
+}
+
+/* B and W from the scratch size: the largest B whose layout with the smallest window fits, then the largest window
+ * (up to the whole buffer) that fits at B, both in window units */
+static bool ip_choose(uint64_t cap, size_t scratch_size, InplaceLayout* L) {
+    for (u32 b = ZXC_BLOCK_SIZE_MAX; b >= ZXC_BLOCK_SIZE_MIN; b >>= 1) {
+        if (!ip_layout(cap, b, 0, L) || L->total > scratch_size) continue;
+        u64 lo = L->W / IP_WINDOW_UNIT, hi = ip_window_max(cap, b) / IP_WINDOW_UNIT;
+        while (lo < hi) {
+            const u64 mid = lo + (hi - lo + 1) / 2;
+            if (ip_layout(cap, b, mid * IP_WINDOW_UNIT, L) && L->total <= scratch_size) lo = mid;
+            else hi = mid - 1;
         }
+        return ip_layout(cap, b, lo * IP_WINDOW_UNIT, L);
     }
-    zxc_dplan_check<<<per_job, DP_THREADS, 0, st>>>(A);
-    zxc_dplan_decide<<<1, 1, 0, st>>>(A);
-    DSplitArgs D;
-    D.a = A;
-    D.dst = (u8*)d_dst;
-    D.slots = base + L.slots;
-    D.scratch = dec;
-    D.dict = d_dict;
-    D.dict_huf = d_huf;
-    D.dict_size = has_dict ? dict_size : 0;
-    D.scratch_stride = scratch_stride_for(bs);
-    D.room = L.room;
-    D.probe_warps = L.probe_warps;
-    const u32 probe_grid = (L.probe_warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-    const u32 dec_grid = (u32)grid_for(L.J);
-    if (has_dict) launch_dsplit<true>(D, 0, probe_grid, st);
-    else launch_dsplit<false>(D, 0, probe_grid, st);
-    zxc_dsplit_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
-    if (has_dict) launch_dsplit<true>(D, 1, dec_grid, st);
-    else launch_dsplit<false>(D, 1, dec_grid, st);
-    zxc_dsplit_final<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
-    __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
+    return false;
+}
+
+extern "C" int zxg_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,
+                                             const void* h_dict, uint32_t dict_size, const void* h_dict_huf,
+                                             uint32_t dict_id, int huf_verdict, int checksum_enabled, void* d_scratch,
+                                             size_t scratch_size, int64_t* d_result, void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    InplaceLayout L;
+    if (!ip_choose(buffer_capacity, scratch_size, &L)) return ZXC_ERROR_MEMORY;
+    const u32 bs = L.bs;
+    const u64 W = L.W;
+    const u32 R = (u32)((comp_size + W - 1) / W);
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    const bool has_dict = h_dict && dict_size;
+    u8 *d_dict, *d_huf;
+    const int drc = dec_stage_dict(base + L.d.dict, h_dict, dict_size, h_dict_huf, st, &d_dict, &d_huf);
+    if (drc != ZXC_OK) return drc;
+    u8* buf = (u8*)d_buffer;
+    const u64 off = buffer_capacity - comp_size; /* the frame lies flush-right */
+    DInplaceArgs I;
+    I.a = dplan_args(base, L.d, buf + off, comp_size, buffer_capacity, bs, has_dict, dict_id, huf_verdict,
+                     checksum_enabled, d_result);
+    I.hazard = (unsigned int*)(base + L.hazard);
+    I.rstart = (unsigned long long*)(base + L.rstart);
+    for (int t = 0; t < 2; t++) {
+        I.rjobs[t] = (zxc_b200_job_t*)(base + L.rjobs[t]);
+        I.rstatus[t] = (i32*)(base + L.rstatus[t]);
+    }
+    I.base = off;
+    I.W = W;
+    I.O = L.O;
+    I.R = R;
+    I.Jr = L.Jr;
+    launch_dplan(I.a, st);
+    zxc_dinplace_probe<<<1, 1, 0, st>>>(I);
+    const u64 plan_threads = (u64)L.d.J > (u64)R + 1 ? L.d.J : (u64)R + 1;
+    zxc_dinplace_plan<<<(u32)((plan_threads + DI_THREADS - 1) / DI_THREADS), DI_THREADS, 0, st>>>(I);
+    __atomic_add_fetch(&g_launches, 2, __ATOMIC_RELAXED);
+    /* round k: frame bytes [k W - 8, min(k W + W + O + 8, comp_size)) into the staging area, frame byte x at
+     * staging + 8 + x - k W, then the round's jobs and their decode from there */
+    u8* staging = base + L.staging;
+    const u32 round_grid = (L.Jr + DI_THREADS - 1) / DI_THREADS;
+    for (u32 k = 0; k < R; k++) {
+        const u64 w = (u64)k * W;
+        const u64 lo = w >= 8 ? w - 8 : 0;
+        const u64 hi = w + W + L.O + 8 < comp_size ? w + W + L.O + 8 : comp_size;
+        if (cudaMemcpyAsync(staging + 8 + lo - w, buf + off + lo, (size_t)(hi - lo), cudaMemcpyDeviceToDevice, st) !=
+            cudaSuccess)
+            return ZXC_B200_ERROR_CUDA;
+        zxc_dinplace_round<<<round_grid, DI_THREADS, 0, st>>>(I, k);
+        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+        const int rc = launch_dplan_decode(staging + 8 - w, buf, I.rjobs[k & 1], I.rstatus[k & 1], L.Jr, I.a.st,
+                                           d_dict, dict_size, d_huf, base + L.d.dec, L.d.dec_bytes, bs,
+                                           checksum_enabled, st);
+        if (rc != ZXC_OK) return rc;
+    }
+    zxc_dinplace_round<<<round_grid, DI_THREADS, 0, st>>>(I, R);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    launch_dplan_verdict(I.a, st);
+    zxc_dinplace_nosplit<<<1, 1, 0, st>>>(I);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    /* the split runs with one round only: the whole frame is then in the staging area */
+    DPlanArgs As = I.a;
+    As.src = staging + 8;
+    launch_dsplit_all(dsplit_args(As, base, L.d, buf, d_dict, d_huf, dict_size, bs), has_dict, st);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 
@@ -1743,21 +1934,9 @@ extern "C" int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uin
     cudaStream_t st = (cudaStream_t)stream;
     u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
     const bool has_dict = h_dict && dict_size;
-    u8* d_dict = NULL;
-    u8* d_huf = NULL;
-    if (has_dict) { /* staged as in zxg_decompress_device */
-        d_dict = base + L.dict;
-        const size_t dbytes = (size_t)dict_size + (h_dict_huf ? ZXC_HUF_TABLE_SIZE : 0);
-        u8* b = (u8*)host_bounce(h_dict, dict_size, dbytes);
-        if (!b) return ZXC_ERROR_MEMORY;
-        if (h_dict_huf) {
-            memcpy(b + dict_size, h_dict_huf, ZXC_HUF_TABLE_SIZE);
-            d_huf = d_dict + dict_size;
-        }
-        const cudaError_t e = cudaMemcpyAsync(d_dict, b, dbytes, cudaMemcpyHostToDevice, st);
-        free(b);
-        if (e != cudaSuccess) return ZXC_B200_ERROR_CUDA;
-    }
+    u8 *d_dict, *d_huf;
+    const int drc = dec_stage_dict(base + L.dict, h_dict, dict_size, h_dict_huf, st, &d_dict, &d_huf);
+    if (drc != ZXC_OK) return drc;
     DBatchState* S = (DBatchState*)base;
     DBatchArgs A;
     A.frames = d_frames;

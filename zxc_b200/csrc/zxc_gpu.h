@@ -82,6 +82,17 @@ int zxg_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uin
                           int huf_verdict, int checksum_enabled, void* d_scratch, size_t scratch_size,
                           int64_t* d_result, void* stream);
 
+/* In-place decode of a device-resident frame (zxc_b200_decompress_inplace_device; kernels in zxc_dinplace.cuh): the
+ * frame of comp_size bytes lies flush-right in d_buffer[0 .. buffer_capacity) and decodes into d_buffer[0 ..).  The
+ * host passes what zxg_decompress_device takes; ZXC_ERROR_MEMORY when the scratch holds less than the layout for 4 KiB
+ * blocks and the smallest window.  The scratch size for a window of `window` compressed bytes per round (0 without a
+ * device or when that cannot be planned). */
+size_t zxg_decompress_inplace_scratch_bytes(uint64_t buffer_capacity, uint32_t block_size, uint64_t window);
+int zxg_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size, const void* h_dict,
+                                  uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id, int huf_verdict,
+                                  int checksum_enabled, void* d_scratch, size_t scratch_size, int64_t* d_result,
+                                  void* stream);
+
 /* Many device-resident frames in one call (zxc_b200_decompress_device_batch; kernels in zxc_dbatch.cuh), with the
  * host's share of the verdicts made as for zxg_decompress_device.  Scratch for up to max_frames frames of at most
  * max_total_capacity output bytes in all and block_size-byte blocks (0 without a device or when that cannot be

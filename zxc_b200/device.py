@@ -6,9 +6,13 @@ compress call emitted.  ``decompress_frame`` decodes any frame held in a uint8 C
 zxc_b200_decompress_device, which plans, decodes and checks it on the device.  ``SeekableFrame`` decodes byte ranges of
 a seekable frame in HBM with zxc_b200_seekable_device_decompress_ranges.  ``decompress_frames`` decodes many frames
 in one zxc_b200_decompress_device_batch call, and ``compress_frames`` compresses many tensors into one frame each in
-one zxc_b200_compress_device_batch call.  Kept apart from ``zxc_b200`` so that importing the package does not import torch.
+one zxc_b200_compress_device_batch call.  ``decompress_inplace`` decodes a frame that lies flush-right in a CUDA buffer
+into the same buffer with zxc_b200_decompress_inplace_device, and ``load_frame`` uses it to bring a frame from the
+host into HBM and expand it there with no second buffer.  Kept apart from ``zxc_b200`` so that importing the package
+does not import torch.
 """
 import ctypes as C
+import warnings
 from dataclasses import dataclass
 
 import torch
@@ -220,6 +224,114 @@ def decompress_frame(frame, *, capacity=None, dict=None, dict_huf=None, checksum
     if r < 0:
         raise ZxcError(r, "zxc_b200_decompress_device")
     return out[:r]
+
+
+lib.zxc_decompress_inplace_bound.restype = C.c_size_t
+lib.zxc_decompress_inplace_bound.argtypes = [C.c_void_p, C.c_size_t]
+lib.zxc_b200_decompress_inplace_device_bound.restype = C.c_size_t
+lib.zxc_b200_decompress_inplace_device_bound.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
+lib.zxc_b200_decompress_inplace_device_scratch_size.restype = C.c_size_t
+lib.zxc_b200_decompress_inplace_device_scratch_size.argtypes = [C.c_uint64, C.c_uint32, C.c_uint64]
+lib.zxc_b200_decompress_inplace_device.restype = C.c_int
+lib.zxc_b200_decompress_inplace_device.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p,
+                                                   C.c_size_t, C.c_void_p, C.c_void_p]
+
+WINDOW_DEFAULT = 256 << 20
+
+
+def _host_bytes(frame):
+    """a host frame (bytes-like or array) as a contiguous uint8 numpy array"""
+    import numpy as np
+    return np.ascontiguousarray(np.frombuffer(frame, np.uint8) if isinstance(frame, (bytes, bytearray, memoryview))
+                                else np.asarray(frame).reshape(-1).view(np.uint8))
+
+
+def inplace_bound(frame, stream=None):
+    """zxc_decompress_inplace_bound: the buffer size that decodes `frame` in place (0 for a frame it rejects).
+
+    `frame` is a contiguous uint8 CUDA tensor (its header and footer are read with zxc_b200_decompress_inplace_device_bound,
+    which synchronises `stream`, default the current stream) or host bytes / an array."""
+    if isinstance(frame, torch.Tensor) and frame.is_cuda:
+        if frame.dtype != torch.uint8 or not frame.is_contiguous():
+            raise ValueError("frame must be a contiguous uint8 CUDA tensor")
+        with torch.cuda.device(frame.device):
+            stream = stream or torch.cuda.current_stream(frame.device)
+            return int(lib.zxc_b200_decompress_inplace_device_bound(frame.data_ptr(), frame.numel(),
+                                                                    stream.cuda_stream))
+    h = _host_bytes(frame.numpy() if isinstance(frame, torch.Tensor) else frame)
+    return int(lib.zxc_decompress_inplace_bound(h.ctypes.data, h.size))
+
+
+def decompress_inplace(buf, comp_size, *, dict=None, dict_huf=None, checksum=False, window=None, stream=None):
+    """Decode the frame of comp_size bytes that lies flush-right in `buf`, a contiguous uint8 CUDA tensor, into the
+    same tensor; returns buf[:n], n the decoded size.
+
+    Runs zxc_b200_decompress_inplace_device on `stream` (default: the current stream of buf's device) and synchronises
+    it once to read the result, which is what zxc_decompress_inplace returns for the same buffer and options; an error
+    raises ZxcError with its exact code (the buffer's contents are then unspecified, except for ZXC_ERROR_MEMORY from
+    the round schedule, which leaves it as it was).  `window` is the compressed bytes staged per round, default
+    min(comp_size, 256 MiB); a window of comp_size decodes in one round unless the scratch it takes reads as one for a
+    larger block size (see zxc_b200_decompress_inplace_device in zxc_b200.h).  Reads the frame's header byte that
+    sizes the scratch with one small copy.  dict / dict_huf are host bytes."""
+    if not buf.is_cuda or buf.dtype != torch.uint8 or not buf.is_contiguous():
+        raise ValueError("buf must be a contiguous uint8 CUDA tensor")
+    b = buf.reshape(-1)
+    cap, comp_size = b.numel(), int(comp_size)
+    o = _DOpts(checksum_enabled=int(bool(checksum)))
+    keep = []
+    if dict is not None:
+        d = bytes(dict)
+        keep.append(d)
+        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+        if dict_huf is not None:
+            h = bytes(dict_huf)
+            keep.append(h)
+            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    window = min(int(window) if window is not None else WINDOW_DEFAULT, comp_size)
+    dev = b.device
+    with torch.cuda.device(dev):
+        stream = stream or torch.cuda.current_stream(dev)
+        with torch.cuda.stream(stream):
+            bs = 4096
+            if 28 <= comp_size <= cap:
+                code = int(b[cap - comp_size + 5].item())
+                bs = 1 << code if 12 <= code <= 21 else 4096
+            scratch_size = int(lib.zxc_b200_decompress_inplace_device_scratch_size(cap, bs, window))
+            if scratch_size == 0:
+                raise ValueError("zxc_b200_decompress_inplace_device_scratch_size: buffer too large, or no device")
+            scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
+            result = torch.empty(1, dtype=torch.int64, device=dev)
+            rc = lib.zxc_b200_decompress_inplace_device(b.data_ptr(), cap, comp_size, C.byref(o), scratch.data_ptr(),
+                                                        scratch_size, result.data_ptr(), stream.cuda_stream)
+            if rc != 0:
+                raise ZxcError(rc, "zxc_b200_decompress_inplace_device")
+            stream.synchronize()
+            r = int(result.item())
+    if r < 0:
+        raise ZxcError(r, "zxc_b200_decompress_inplace_device")
+    return b[:r]
+
+
+def load_frame(frame, *, device=None, dict=None, dict_huf=None, checksum=False, window=None, stream=None):
+    """Bring a ZXC frame from host memory (bytes or an array) into HBM and decode it there in place; returns a uint8
+    CUDA tensor of the decoded bytes.
+
+    Allocates one buffer of zxc_decompress_inplace_bound bytes on `device` (default: the current CUDA device), copies
+    the frame to its end and runs decompress_inplace on it: the device memory taken is that buffer and the decode's
+    scratch, with no separate copy of the compressed frame.  The result is a view of the buffer.  A frame the bound
+    rejects is decoded in a buffer of its own size, so it raises ZxcError with zxc_decompress_inplace's code for it."""
+    h = _host_bytes(frame)
+    bound = int(lib.zxc_decompress_inplace_bound(h.ctypes.data, h.size)) or max(h.size, 1)
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    with torch.cuda.device(dev):
+        stream = stream or torch.cuda.current_stream(dev)
+        with torch.cuda.stream(stream):
+            buf = torch.empty(bound, dtype=torch.uint8, device=dev)
+            with warnings.catch_warnings():  # a frame from bytes is read-only; it is only read
+                warnings.simplefilter("ignore")
+                buf[bound - h.size:].copy_(torch.from_numpy(h))
+    return decompress_inplace(buf, h.size, dict=dict, dict_huf=dict_huf, checksum=checksum, window=window,
+                              stream=stream)
 
 
 lib.zxc_b200_decompress_device_batch_scratch_size.restype = C.c_size_t
