@@ -1015,6 +1015,21 @@ size_t zxc_b200_decompress_device_scratch_size(uint64_t dst_capacity, uint32_t b
     return zxg_decompress_scratch_bytes(dst_capacity, block_size);
 }
 
+/* The decode options of the device-resident decodes: decompress_frame's dictionary checks that need no frame bytes */
+static int device_dopts(const zxc_decompress_opts_t* opts, zxg_dopts_t* o) {
+    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
+    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    o->dict = dict_size ? dict : NULL;
+    o->dict_size = (uint32_t)dict_size;
+    o->dict_id = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
+    o->huf_verdict = dict_size ? dict_huf_attach(dict_huf) : 0;
+    o->dict_huf = o->huf_verdict == 1 ? dict_huf : NULL;
+    o->checksum_enabled = opts ? opts->checksum_enabled : 0;
+    return ZXC_OK;
+}
+
 /* The host decides what needs no frame bytes, in zxc_decompress's order (decompress_entry, decompress_frame); the
  * device decides the rest and writes it to *d_result (zxc_dplan.cuh). */
 int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
@@ -1022,17 +1037,12 @@ int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst
                                int64_t* d_result, void* stream) {
     if (!d_src || (!d_dst && dst_capacity != 0) || !d_scratch || !d_result) return ZXC_ERROR_NULL_INPUT;
     if (src_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE) return ZXC_ERROR_SRC_TOO_SMALL;
-    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
-    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
-    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
-    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    zxg_dopts_t o;
+    const int orc = device_dopts(opts, &o);
+    if (orc != ZXC_OK) return orc;
     const int irc = zxg_init();
     if (irc != ZXC_OK) return irc;
-    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
-    const int arc = dict_size ? dict_huf_attach(dict_huf) : 0;
-    return zxg_decompress_device(d_src, src_size, d_dst, dst_capacity, dict_size ? dict : NULL, (uint32_t)dict_size,
-                                 arc == 1 ? dict_huf : NULL, did, arc, opts ? opts->checksum_enabled : 0, d_scratch,
-                                 scratch_size, d_result, stream);
+    return zxg_decompress_device(d_src, src_size, d_dst, dst_capacity, &o, d_scratch, scratch_size, d_result, stream);
 }
 
 size_t zxc_b200_decompress_inplace_device_scratch_size(uint64_t buffer_capacity, uint32_t block_size, uint64_t window) {
@@ -1057,17 +1067,13 @@ int zxc_b200_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity,
     if (!d_buffer || comp_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE || comp_size > buffer_capacity ||
         !d_scratch || !d_result)
         return ZXC_ERROR_NULL_INPUT;
-    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
-    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
-    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
-    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    zxg_dopts_t o;
+    const int orc = device_dopts(opts, &o);
+    if (orc != ZXC_OK) return orc;
     const int irc = zxg_init();
     if (irc != ZXC_OK) return irc;
-    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
-    const int arc = dict_size ? dict_huf_attach(dict_huf) : 0;
-    return zxg_decompress_inplace_device(d_buffer, buffer_capacity, comp_size, dict_size ? dict : NULL,
-                                         (uint32_t)dict_size, arc == 1 ? dict_huf : NULL, did, arc,
-                                         opts ? opts->checksum_enabled : 0, d_scratch, scratch_size, d_result, stream);
+    return zxg_decompress_inplace_device(d_buffer, buffer_capacity, comp_size, &o, d_scratch, scratch_size, d_result,
+                                         stream);
 }
 
 size_t zxc_b200_decompress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_capacity,
@@ -1082,17 +1088,12 @@ int zxc_b200_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t 
                                      const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
                                      int64_t* d_results, void* stream) {
     if (n_frames > 0 && (!d_frames || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
-    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
-    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
-    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
-    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    zxg_dopts_t o;
+    const int orc = device_dopts(opts, &o);
+    if (orc != ZXC_OK) return orc;
     const int irc = zxg_init();
     if (irc != ZXC_OK || n_frames == 0) return irc;
-    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
-    const int arc = dict_size ? dict_huf_attach(dict_huf) : 0;
-    return zxg_decompress_device_batch(d_frames, n_frames, dict_size ? dict : NULL, (uint32_t)dict_size,
-                                       arc == 1 ? dict_huf : NULL, did, arc, opts ? opts->checksum_enabled : 0,
-                                       d_scratch, scratch_size, d_results, stream);
+    return zxg_decompress_device_batch(d_frames, n_frames, &o, d_scratch, scratch_size, d_results, stream);
 }
 
 int64_t zxc_compress_cctx(zxc_cctx* cctx, const void* src, size_t src_size, void* dst, size_t dst_capacity,

@@ -14,7 +14,8 @@
  *   zxc_dinplace_round(R) the last round's statuses
  *   zxc_dplan_check / _decide  (unchanged)
  *   zxc_dinplace_nosplit  with more than one round, a frame that needs the general split gets ZXC_ERROR_MEMORY
- *   zxc_dsplit_*          (unchanged) the general split, reading the staged copy (one round only)
+ *   zxc_dsplit_*          (unchanged) the general split, reading the staged copy (one round only: its DSplitArgs
+ *                         source base is the staging area)
  *
  * Rounds: the frame is cut into windows [k W, (k + 1) W) of compressed bytes, W fixed on the host from the scratch, so
  * R = ceil(comp_size / W).  A job belongs to the round whose window holds its block header; round k's staged copy is
@@ -105,7 +106,7 @@ __global__ void __launch_bounds__(DI_THREADS) zxc_dinplace_plan(const DInplaceAr
 }
 
 /* round k: gather round k - 1's statuses (k > 0), then place round k's jobs (k < R) right-aligned in table k & 1 and
- * preset the decode counters as zxc_dplan_place does for the whole frame.  The hazard verdict is written here, before
+ * preset the decode counters (dp_slot, dp_preset) as zxc_dplan_place does for the whole frame.  The hazard verdict is written here, before
  * round 0's decode. */
 __global__ void __launch_bounds__(DI_THREADS) zxc_dinplace_round(const DInplaceArgs I, const u32 k) {
     const DPlanArgs& A = I.a;
@@ -133,12 +134,8 @@ __global__ void __launch_bounds__(DI_THREADS) zxc_dinplace_round(const DInplaceA
         else if (i < Jr) I.rjobs[k & 1][i] = A.jobs[first + a + (i - (Jr - n))];
     }
     if (i == 0) {
-        const u32 slot = live ? (__ffs(S->block_size) - 1 - ZXC_BLOCK_SIZE_MIN_LOG2) * 2 + S->verify : DP_SLOTS;
-        for (u32 t = 0; t < DP_SLOTS; t++) {
-            S->ctr[t][0] = t == slot ? Jr - n : Jr;
-            S->ctr[t][1] = 0;
-            S->ctr[t][2] = 0;
-        }
+        const u32 slot = live ? dp_slot(S) : DP_SLOTS;
+        for (u32 t = 0; t < DP_SLOTS; t++) dp_preset(S->ctr[t], t == slot ? Jr - n : Jr);
     }
 }
 

@@ -1498,22 +1498,113 @@ extern "C" int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint3
 /* A decode's dictionary and its literal table (when given) into the scratch's dictionary region at d_region, through
  * a pageable host copy: the caller's dictionary has been read when the call returns, whatever memory it is in
  * (host_bounce).  Both device pointers stay NULL without a dictionary. */
-static int dec_stage_dict(u8* d_region, const void* h_dict, u32 dict_size, const void* h_dict_huf, cudaStream_t st,
-                          u8** d_dict, u8** d_huf) {
+static int dec_stage_dict(u8* d_region, const zxg_dopts_t* o, cudaStream_t st, u8** d_dict, u8** d_huf) {
     *d_dict = NULL;
     *d_huf = NULL;
-    if (!h_dict || !dict_size) return ZXC_OK;
+    const u32 dict_size = o->dict_size;
+    if (!o->dict || !dict_size) return ZXC_OK;
     *d_dict = d_region;
-    const size_t dbytes = (size_t)dict_size + (h_dict_huf ? ZXC_HUF_TABLE_SIZE : 0);
-    u8* b = (u8*)host_bounce(h_dict, dict_size, dbytes);
+    const size_t dbytes = (size_t)dict_size + (o->dict_huf ? ZXC_HUF_TABLE_SIZE : 0);
+    u8* b = (u8*)host_bounce(o->dict, dict_size, dbytes);
     if (!b) return ZXC_ERROR_MEMORY;
-    if (h_dict_huf) {
-        memcpy(b + dict_size, h_dict_huf, ZXC_HUF_TABLE_SIZE);
+    if (o->dict_huf) {
+        memcpy(b + dict_size, o->dict_huf, ZXC_HUF_TABLE_SIZE);
         *d_huf = d_region + dict_size;
     }
     const cudaError_t e = cudaMemcpyAsync(d_region, b, dbytes, cudaMemcpyHostToDevice, st);
     free(b);
     return e == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* the device's share of the decode options, for a scratch sized for block size bs */
+static DDecodeOpts dec_opts(const zxg_dopts_t* o, u32 bs) {
+    DDecodeOpts d;
+    d.max_block_size = bs;
+    d.dict_id = o->dict_id;
+    d.have_dict = o->dict && o->dict_size ? 1u : 0u;
+    d.huf_verdict = o->huf_verdict;
+    d.checksum_enabled = o->checksum_enabled ? 1u : 0u;
+    return d;
+}
+
+/* the largest v in [lo, hi] with fits(v), given fits(lo) and a fits that holds up to some value and not beyond: how
+ * the calls below size their tables and windows to the scratch they are given */
+template <class Fits>
+static u64 largest_fit(u64 lo, u64 hi, Fits fits) {
+    while (lo < hi) {
+        const u64 mid = lo + (hi - lo + 1) / 2;
+        if (fits(mid)) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+/* the largest block size b with fits(b) (0: none) */
+template <class Fits>
+static u32 largest_block_size(Fits fits) {
+    for (u32 b = ZXC_BLOCK_SIZE_MAX; b >= ZXC_BLOCK_SIZE_MIN; b >>= 1)
+        if (fits(b)) return b;
+    return 0;
+}
+
+/* the general split's size probe (a rare path): one slot of bs + ZXF_TAIL_PAD per warp of the decode grid for
+ * grid_jobs jobs, at most 256 MiB of them and at most J; returns the slots' bytes in the layout */
+static size_t split_probe_slots(u32 bs, u32 grid_jobs, u64 J, u32* room, u32* probe_warps) {
+    *room = bs + ZXF_TAIL_PAD;
+    const u32 dec_warps = (u32)grid_for(grid_jobs) * WARPS_PER_CTA;
+    const u32 by_room = (u32)(((size_t)256 << 20) / *room);
+    u64 pw = dec_warps < by_room ? dec_warps : by_room;
+    if (pw > J) pw = J;
+    *probe_warps = pw ? (u32)pw : 1;
+    return r256((size_t)*probe_warps * *room);
+}
+
+/* the general split's decode arguments: the plan's bases src and dst, its probe slots and the decode scratch */
+static DSplitArgs split_args(const void* src, void* dst, u8* slots, u8* dec, const u8* d_dict, const u8* d_huf,
+                             const zxg_dopts_t* o, u32 bs, u32 room, u32 probe_warps) {
+    DSplitArgs D;
+    D.src = (const u8*)src;
+    D.dst = (u8*)dst;
+    D.slots = slots;
+    D.scratch = dec;
+    D.dict = d_dict;
+    D.dict_huf = d_huf;
+    D.dict_size = d_dict ? o->dict_size : 0;
+    D.scratch_stride = scratch_stride_for(bs);
+    D.room = room;
+    D.probe_warps = probe_warps;
+    return D;
+}
+
+/* the general split's four launches for either kernel family (zxc_dplan.cuh, zxc_dbatch.cuh); they exit at once
+ * unless a frame split */
+template <class Ar>
+static void launch_split(void (*decode)(Ar, DSplitArgs, u32), void (*scan)(Ar), void (*final)(Ar), const Ar& A,
+                         const DSplitArgs& D, u32 dec_grid, u32 scan_grid, cudaStream_t st) {
+    const u32 probe_grid = (D.probe_warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
+    decode<<<probe_grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(A, D, 0);
+    scan<<<scan_grid, ASM_SCAN_THREADS, 0, st>>>(A);
+    decode<<<dec_grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(A, D, 1);
+    final<<<scan_grid, ASM_SCAN_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 4, __ATOMIC_RELAXED);
+}
+
+/* one launch_decode per launch slot: block sizes up to bs, checksum verification off / on.  Slot s's jobs and status
+ * words start at entry s * stride (stride 0: one table of n_jobs for every slot); only the slots with work have
+ * counters preset below J on the device. */
+static int launch_slot_decodes(const void* d_src, void* d_dst, const zxc_b200_job_t* jobs, i32* status, u32 n_jobs,
+                               u64 stride, unsigned long long (*ctr)[4], const u8* d_dict, const u8* d_huf,
+                               const zxg_dopts_t* o, u8* dec, size_t dec_bytes, u32 bs, cudaStream_t st) {
+    for (u32 b = ZXC_BLOCK_SIZE_MIN; b <= bs; b <<= 1) {
+        const u32 lg = (u32)__builtin_ctz(b) - ZXC_BLOCK_SIZE_MIN_LOG2;
+        for (int v = 0; v <= (o->checksum_enabled ? 1 : 0); v++) {
+            const u32 slot = lg * 2 + v;
+            const int rc = launch_decode(d_src, d_dst, jobs + slot * stride, n_jobs, status + slot * stride, d_dict,
+                                         o->dict_size, d_huf, dec, dec_bytes, b, v, ctr[slot], st, 1);
+            if (rc != ZXC_OK) return rc;
+        }
+    }
+    return ZXC_OK;
 }
 
 struct DevDecLayout {
@@ -1537,15 +1628,8 @@ static bool dev_dec_layout(uint64_t dst_capacity, u32 block_size, DevDecLayout* 
     o += r256((size_t)J * 4);
     L->tiles = o;
     o += r256(((size_t)J + ASM_TILE - 1) / ASM_TILE * 8);
-    /* the split's size probe: one slot of block_size + ZXF_TAIL_PAD per warp, at most 256 MiB of them (a rare path) */
-    L->room = block_size + ZXF_TAIL_PAD;
-    const u32 dec_warps = (u32)grid_for(J) * WARPS_PER_CTA;
-    const u32 by_room = (u32)(((size_t)256 << 20) / L->room);
-    u32 pw = dec_warps < by_room ? dec_warps : by_room;
-    if (pw > J) pw = J;
-    L->probe_warps = pw ? pw : 1;
     L->slots = o;
-    o += r256((size_t)L->probe_warps * L->room);
+    o += split_probe_slots(block_size, J, J, &L->room, &L->probe_warps);
     L->dec = o;
     L->dec_bytes = launch_scratch_bytes(J, block_size);
     o += L->dec_bytes;
@@ -1560,28 +1644,9 @@ extern "C" size_t zxg_decompress_scratch_bytes(uint64_t dst_capacity, uint32_t b
     return dev_dec_layout(dst_capacity, block_size, &L) ? L.total : 0;
 }
 
-template <bool HAS_DICT>
-static void launch_dsplit(const DSplitArgs& D, u32 phase, u32 grid, cudaStream_t st) {
-    zxc_dsplit_decode<HAS_DICT><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(D, phase);
-}
-
-/* the general split's four launches (zxc_dplan.cuh); they exit at once unless zxc_dplan_decide asked for it */
-static void launch_dsplit_all(const DSplitArgs& D, bool has_dict, cudaStream_t st) {
-    const u32 probe_grid = (D.probe_warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-    const u32 dec_grid = (u32)grid_for(D.a.J);
-    if (has_dict) launch_dsplit<true>(D, 0, probe_grid, st);
-    else launch_dsplit<false>(D, 0, probe_grid, st);
-    zxc_dsplit_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(D.a);
-    if (has_dict) launch_dsplit<true>(D, 1, dec_grid, st);
-    else launch_dsplit<false>(D, 1, dec_grid, st);
-    zxc_dsplit_final<<<1, ASM_SCAN_THREADS, 0, st>>>(D.a);
-    __atomic_add_fetch(&g_launches, 4, __ATOMIC_RELAXED);
-}
-
 /* zxc_dplan.cuh's arguments over a DevDecLayout at base */
 static DPlanArgs dplan_args(u8* base, const DevDecLayout& L, const void* d_src, uint64_t src_size,
-                            uint64_t dst_capacity, u32 bs, bool has_dict, uint32_t dict_id, int huf_verdict,
-                            int checksum_enabled, int64_t* d_result) {
+                            uint64_t dst_capacity, u32 bs, const zxg_dopts_t* o, int64_t* d_result) {
     DPlanArgs A;
     A.src = (const u8*)d_src;
     A.src_size = src_size;
@@ -1594,11 +1659,7 @@ static DPlanArgs dplan_args(u8* base, const DevDecLayout& L, const void* d_src, 
     A.st = (DPlanState*)base;
     A.result = (long long*)d_result;
     A.J = L.J;
-    A.max_block_size = bs;
-    A.dict_id = dict_id;
-    A.have_dict = has_dict ? 1u : 0u;
-    A.huf_verdict = huf_verdict;
-    A.checksum_enabled = checksum_enabled ? 1u : 0u;
+    A.o = dec_opts(o, bs);
     return A;
 }
 
@@ -1615,39 +1676,6 @@ static void launch_dplan(const DPlanArgs& A, cudaStream_t st) {
     __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
 }
 
-/* one launch_decode per slot: block sizes up to bs, checksum verification off / on; only the frame's has work.  The
- * job table has J entries and the counters were preset on the device. */
-static int launch_dplan_decode(const void* d_src, void* d_dst, const zxc_b200_job_t* jobs, i32* status, u32 J,
-                               DPlanState* S, const u8* d_dict, u32 dict_size, const u8* d_huf, u8* dec,
-                               size_t dec_bytes, u32 bs, int checksum_enabled, cudaStream_t st) {
-    for (u32 b = ZXC_BLOCK_SIZE_MIN; b <= bs; b <<= 1) {
-        const u32 lg = (u32)__builtin_ctz(b) - ZXC_BLOCK_SIZE_MIN_LOG2;
-        for (int v = 0; v <= (checksum_enabled ? 1 : 0); v++) {
-            const int rc = launch_decode(d_src, d_dst, jobs, J, status, d_dict, dict_size, d_huf, dec, dec_bytes, b,
-                                         v, S->ctr[lg * 2 + v], st, 1);
-            if (rc != ZXC_OK) return rc;
-        }
-    }
-    return ZXC_OK;
-}
-
-/* the general split's arguments over a DevDecLayout at base */
-static DSplitArgs dsplit_args(const DPlanArgs& A, u8* base, const DevDecLayout& L, void* d_dst, u8* d_dict,
-                              u8* d_huf, u32 dict_size, u32 bs) {
-    DSplitArgs D;
-    D.a = A;
-    D.dst = (u8*)d_dst;
-    D.slots = base + L.slots;
-    D.scratch = base + L.dec;
-    D.dict = d_dict;
-    D.dict_huf = d_huf;
-    D.dict_size = d_dict ? dict_size : 0;
-    D.scratch_stride = scratch_stride_for(bs);
-    D.room = L.room;
-    D.probe_warps = L.probe_warps;
-    return D;
-}
-
 /* the first failing job, then zxc_decompress's verdict or the general split's go-ahead */
 static void launch_dplan_verdict(const DPlanArgs& A, cudaStream_t st) {
     zxc_dplan_check<<<(A.J + DP_THREADS - 1) / DP_THREADS, DP_THREADS, 0, st>>>(A);
@@ -1655,36 +1683,38 @@ static void launch_dplan_verdict(const DPlanArgs& A, cudaStream_t st) {
     __atomic_add_fetch(&g_launches, 2, __ATOMIC_RELAXED);
 }
 
+/* the single frame's general split, its plan's offsets over src and dst */
+static void launch_dsplit(const DPlanArgs& A, const DevDecLayout& L, u8* base, const void* src, void* dst,
+                          const u8* d_dict, const u8* d_huf, const zxg_dopts_t* o, u32 bs, cudaStream_t st) {
+    const DSplitArgs D = split_args(src, dst, base + L.slots, base + L.dec, d_dict, d_huf, o, bs, L.room,
+                                    L.probe_warps);
+    launch_split(d_dict ? zxc_dsplit_decode<true> : zxc_dsplit_decode<false>, zxc_dsplit_scan, zxc_dsplit_final, A,
+                 D, (u32)grid_for(L.J), 1, st);
+}
+
 extern "C" int zxg_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
-                                     const void* h_dict, uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id,
-                                     int huf_verdict, int checksum_enabled, void* d_scratch, size_t scratch_size,
-                                     int64_t* d_result, void* stream) {
+                                     const zxg_dopts_t* o, void* d_scratch, size_t scratch_size, int64_t* d_result,
+                                     void* stream) {
     const int irc = zxg_init();
     if (irc != ZXC_OK) return irc;
     /* the largest block size this scratch was sized for */
-    u32 bs = 0;
     DevDecLayout L;
-    for (u32 b = ZXC_BLOCK_SIZE_MAX; b >= ZXC_BLOCK_SIZE_MIN; b >>= 1) {
-        if (dev_dec_layout(dst_capacity, b, &L) && L.total <= scratch_size) {
-            bs = b;
-            break;
-        }
-    }
+    const u32 bs = largest_block_size([&](u32 b) {
+        return dev_dec_layout(dst_capacity, b, &L) && L.total <= scratch_size;
+    });
     if (!bs) return ZXC_ERROR_MEMORY;
     cudaStream_t st = (cudaStream_t)stream;
     u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
-    const bool has_dict = h_dict && dict_size;
     u8 *d_dict, *d_huf;
-    const int drc = dec_stage_dict(base + L.dict, h_dict, dict_size, h_dict_huf, st, &d_dict, &d_huf);
+    const int drc = dec_stage_dict(base + L.dict, o, st, &d_dict, &d_huf);
     if (drc != ZXC_OK) return drc;
-    const DPlanArgs A = dplan_args(base, L, d_src, src_size, dst_capacity, bs, has_dict, dict_id, huf_verdict,
-                                   checksum_enabled, d_result);
+    const DPlanArgs A = dplan_args(base, L, d_src, src_size, dst_capacity, bs, o, d_result);
     launch_dplan(A, st);
-    const int rc = launch_dplan_decode(d_src, d_dst, A.jobs, A.status, L.J, A.st, d_dict, dict_size, d_huf,
-                                       base + L.dec, L.dec_bytes, bs, checksum_enabled, st);
+    const int rc = launch_slot_decodes(d_src, d_dst, A.jobs, A.status, L.J, 0, A.st->ctr, d_dict, d_huf, o,
+                                       base + L.dec, L.dec_bytes, bs, st);
     if (rc != ZXC_OK) return rc;
     launch_dplan_verdict(A, st);
-    launch_dsplit_all(dsplit_args(A, base, L, d_dst, d_dict, d_huf, dict_size, bs), has_dict, st);
+    launch_dsplit(A, L, base, d_src, d_dst, d_dict, d_huf, o, bs, st);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 
@@ -1749,23 +1779,17 @@ extern "C" size_t zxg_decompress_inplace_scratch_bytes(uint64_t buffer_capacity,
 /* B and W from the scratch size: the largest B whose layout with the smallest window fits, then the largest window
  * (up to the whole buffer) that fits at B, both in window units */
 static bool ip_choose(uint64_t cap, size_t scratch_size, InplaceLayout* L) {
-    for (u32 b = ZXC_BLOCK_SIZE_MAX; b >= ZXC_BLOCK_SIZE_MIN; b >>= 1) {
-        if (!ip_layout(cap, b, 0, L) || L->total > scratch_size) continue;
-        u64 lo = L->W / IP_WINDOW_UNIT, hi = ip_window_max(cap, b) / IP_WINDOW_UNIT;
-        while (lo < hi) {
-            const u64 mid = lo + (hi - lo + 1) / 2;
-            if (ip_layout(cap, b, mid * IP_WINDOW_UNIT, L) && L->total <= scratch_size) lo = mid;
-            else hi = mid - 1;
-        }
-        return ip_layout(cap, b, lo * IP_WINDOW_UNIT, L);
-    }
-    return false;
+    const auto fits = [&](u32 b, u64 W) { return ip_layout(cap, b, W, L) && L->total <= scratch_size; };
+    const u32 bs = largest_block_size([&](u32 b) { return fits(b, 0); });
+    if (!bs) return false;
+    const u64 units = largest_fit(L->W / IP_WINDOW_UNIT, ip_window_max(cap, bs) / IP_WINDOW_UNIT,
+                                  [&](u64 u) { return fits(bs, u * IP_WINDOW_UNIT); });
+    return ip_layout(cap, bs, units * IP_WINDOW_UNIT, L);
 }
 
 extern "C" int zxg_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,
-                                             const void* h_dict, uint32_t dict_size, const void* h_dict_huf,
-                                             uint32_t dict_id, int huf_verdict, int checksum_enabled, void* d_scratch,
-                                             size_t scratch_size, int64_t* d_result, void* stream) {
+                                             const zxg_dopts_t* o, void* d_scratch, size_t scratch_size,
+                                             int64_t* d_result, void* stream) {
     const int irc = zxg_init();
     if (irc != ZXC_OK) return irc;
     InplaceLayout L;
@@ -1775,15 +1799,13 @@ extern "C" int zxg_decompress_inplace_device(void* d_buffer, uint64_t buffer_cap
     const u32 R = (u32)((comp_size + W - 1) / W);
     cudaStream_t st = (cudaStream_t)stream;
     u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
-    const bool has_dict = h_dict && dict_size;
     u8 *d_dict, *d_huf;
-    const int drc = dec_stage_dict(base + L.d.dict, h_dict, dict_size, h_dict_huf, st, &d_dict, &d_huf);
+    const int drc = dec_stage_dict(base + L.d.dict, o, st, &d_dict, &d_huf);
     if (drc != ZXC_OK) return drc;
     u8* buf = (u8*)d_buffer;
     const u64 off = buffer_capacity - comp_size; /* the frame lies flush-right */
     DInplaceArgs I;
-    I.a = dplan_args(base, L.d, buf + off, comp_size, buffer_capacity, bs, has_dict, dict_id, huf_verdict,
-                     checksum_enabled, d_result);
+    I.a = dplan_args(base, L.d, buf + off, comp_size, buffer_capacity, bs, o, d_result);
     I.hazard = (unsigned int*)(base + L.hazard);
     I.rstart = (unsigned long long*)(base + L.rstart);
     for (int t = 0; t < 2; t++) {
@@ -1813,9 +1835,8 @@ extern "C" int zxg_decompress_inplace_device(void* d_buffer, uint64_t buffer_cap
             return ZXC_B200_ERROR_CUDA;
         zxc_dinplace_round<<<round_grid, DI_THREADS, 0, st>>>(I, k);
         __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
-        const int rc = launch_dplan_decode(staging + 8 - w, buf, I.rjobs[k & 1], I.rstatus[k & 1], L.Jr, I.a.st,
-                                           d_dict, dict_size, d_huf, base + L.d.dec, L.d.dec_bytes, bs,
-                                           checksum_enabled, st);
+        const int rc = launch_slot_decodes(staging + 8 - w, buf, I.rjobs[k & 1], I.rstatus[k & 1], L.Jr, 0,
+                                           I.a.st->ctr, d_dict, d_huf, o, base + L.d.dec, L.d.dec_bytes, bs, st);
         if (rc != ZXC_OK) return rc;
     }
     zxc_dinplace_round<<<round_grid, DI_THREADS, 0, st>>>(I, R);
@@ -1824,9 +1845,7 @@ extern "C" int zxg_decompress_inplace_device(void* d_buffer, uint64_t buffer_cap
     zxc_dinplace_nosplit<<<1, 1, 0, st>>>(I);
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     /* the split runs with one round only: the whole frame is then in the staging area */
-    DPlanArgs As = I.a;
-    As.src = staging + 8;
-    launch_dsplit_all(dsplit_args(As, base, L.d, buf, d_dict, d_huf, dict_size, bs), has_dict, st);
+    launch_dsplit(I.a, L.d, base, staging + 8, buf, d_dict, d_huf, o, bs, st);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 
@@ -1872,15 +1891,8 @@ static void db_layout(u32 n, u64 Jt, u32 bs, DBatchLayout* L) {
     o += r256((size_t)L->n_slots * Jt * sizeof(zxc_b200_job_t));
     L->status = o;
     o += r256((size_t)L->n_slots * Jt * 4);
-    /* the split's size probe: one slot of bs + ZXF_TAIL_PAD per warp, at most 256 MiB of them (a rare path) */
-    L->room = bs + ZXF_TAIL_PAD;
-    const u32 dec_warps = (u32)grid_for((u32)DB_J_MAX) * WARPS_PER_CTA;
-    const u32 by_room = (u32)(((size_t)256 << 20) / L->room);
-    u64 pw = dec_warps < by_room ? dec_warps : by_room;
-    if (pw > Jt) pw = Jt;
-    L->probe_warps = pw ? (u32)pw : 1;
     L->slots = o;
-    o += r256((size_t)L->probe_warps * L->room);
+    o += split_probe_slots(bs, (u32)DB_J_MAX, Jt, &L->room, &L->probe_warps);
     L->dec = o;
     L->dec_bytes = launch_scratch_bytes((u32)DB_J_MAX, bs);
     L->total = o + L->dec_bytes + 256; /* base alignment slack */
@@ -1898,44 +1910,26 @@ extern "C" size_t zxg_decompress_batch_scratch_bytes(uint32_t max_frames, uint64
     return L.total;
 }
 
-template <bool HAS_DICT>
-static void launch_dbatch_split(const DBatchSplitArgs& D, u32 phase, u32 grid, cudaStream_t st) {
-    zxc_dbatch_split<HAS_DICT><<<grid, CTA_THREADS, DECODE_SMEM_BYTES, st>>>(D, phase);
-}
-
-extern "C" int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const void* h_dict,
-                                           uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id,
-                                           int huf_verdict, int checksum_enabled, void* d_scratch,
-                                           size_t scratch_size, int64_t* d_results, void* stream) {
+extern "C" int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const zxg_dopts_t* o,
+                                           void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
     const int irc = zxg_init();
     if (irc != ZXC_OK) return irc;
     const u32 n = n_frames;
     if (n > DB_FRAMES_MAX) return ZXC_ERROR_MEMORY;
     const u64 J_min = 3ull * n;
     /* the largest block size whose layout with the smallest table fits, then the largest table at it */
-    u32 bs = 0;
     DBatchLayout L;
-    for (u32 b = ZXC_BLOCK_SIZE_MAX; b >= ZXC_BLOCK_SIZE_MIN; b >>= 1) {
-        db_layout(n, J_min, b, &L);
-        if (L.total <= scratch_size) {
-            bs = b;
-            break;
-        }
-    }
+    const auto fits = [&](u32 b, u64 Jt) {
+        db_layout(n, Jt, b, &L);
+        return L.total <= scratch_size;
+    };
+    const u32 bs = largest_block_size([&](u32 b) { return fits(b, J_min); });
     if (!bs) return ZXC_ERROR_MEMORY;
-    u64 lo = J_min, hi = DB_J_MAX;
-    while (lo < hi) {
-        const u64 mid = lo + (hi - lo + 1) / 2;
-        db_layout(n, mid, bs, &L);
-        if (L.total <= scratch_size) lo = mid;
-        else hi = mid - 1;
-    }
-    db_layout(n, lo, bs, &L);
+    db_layout(n, largest_fit(J_min, DB_J_MAX, [&](u64 Jt) { return fits(bs, Jt); }), bs, &L);
     cudaStream_t st = (cudaStream_t)stream;
     u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
-    const bool has_dict = h_dict && dict_size;
     u8 *d_dict, *d_huf;
-    const int drc = dec_stage_dict(base + L.dict, h_dict, dict_size, h_dict_huf, st, &d_dict, &d_huf);
+    const int drc = dec_stage_dict(base + L.dict, o, st, &d_dict, &d_huf);
     if (drc != ZXC_OK) return drc;
     DBatchState* S = (DBatchState*)base;
     DBatchArgs A;
@@ -1953,11 +1947,7 @@ extern "C" int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uin
     A.Jt = L.Jt;
     A.n = n;
     A.n_slots = L.n_slots;
-    A.max_block_size = bs;
-    A.dict_id = dict_id;
-    A.have_dict = has_dict ? 1u : 0u;
-    A.huf_verdict = huf_verdict;
-    A.checksum_enabled = checksum_enabled ? 1u : 0u;
+    A.o = dec_opts(o, bs);
     const u32 n_tiles = (n + ASM_TILE - 1) / ASM_TILE;
     const u32 per_frame = (n + DB_THREADS - 1) / DB_THREADS;
     const u32 per_cta = n < 4096 ? n : 4096; /* grid-stride over frames, one CTA each */
@@ -1973,40 +1963,18 @@ extern "C" int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uin
     zxc_dbatch_place<<<per_entry, DB_THREADS, 0, st>>>(A);
     __atomic_add_fetch(&g_launches, 8, __ATOMIC_RELAXED);
     if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
-    /* one launch slot per block size up to bs, and per checksum verification off / on, each over its own window */
+    /* each launch slot over its own window */
     u8* dec = base + L.dec;
-    for (u32 b = ZXC_BLOCK_SIZE_MIN; b <= bs; b <<= 1) {
-        const u32 lg = (u32)__builtin_ctz(b) - ZXC_BLOCK_SIZE_MIN_LOG2;
-        for (int v = 0; v <= (checksum_enabled ? 1 : 0); v++) {
-            const u32 slot = lg * 2 + v;
-            const int rc = launch_decode(NULL, NULL, A.jobs + slot * L.Jt, (u32)L.Jt, A.status + slot * L.Jt, d_dict,
-                                         dict_size, d_huf, dec, L.dec_bytes, b, v, S->ctr[slot], st, 1);
-            if (rc != ZXC_OK) return rc;
-        }
-    }
+    const int rc = launch_slot_decodes(NULL, NULL, A.jobs, A.status, (u32)L.Jt, L.Jt, S->ctr, d_dict, d_huf, o, dec,
+                                       L.dec_bytes, bs, st);
+    if (rc != ZXC_OK) return rc;
     zxc_dbatch_check<<<per_entry, DB_THREADS, 0, st>>>(A);
     zxc_dbatch_decide<<<per_frame, DB_THREADS, 0, st>>>(A);
-    DBatchSplitArgs D;
-    D.a = A;
-    D.zero = NULL;
-    D.slots = base + L.slots;
-    D.scratch = dec;
-    D.dict = d_dict;
-    D.dict_huf = d_huf;
-    D.dict_size = has_dict ? dict_size : 0;
-    D.scratch_stride = scratch_stride_for(bs);
-    D.room = L.room;
-    D.probe_warps = L.probe_warps;
-    const u32 probe_grid = (L.probe_warps + WARPS_PER_CTA - 1) / WARPS_PER_CTA;
-    const u32 dec_grid = (u32)grid_for((u32)L.Jt);
-    const u32 split_ctas = n < 1024 ? n : 1024;
-    if (has_dict) launch_dbatch_split<true>(D, 0, probe_grid, st);
-    else launch_dbatch_split<false>(D, 0, probe_grid, st);
-    zxc_dbatch_split_scan<<<split_ctas, ASM_SCAN_THREADS, 0, st>>>(A);
-    if (has_dict) launch_dbatch_split<true>(D, 1, dec_grid, st);
-    else launch_dbatch_split<false>(D, 1, dec_grid, st);
-    zxc_dbatch_split_final<<<split_ctas, ASM_SCAN_THREADS, 0, st>>>(A);
-    __atomic_add_fetch(&g_launches, 6, __ATOMIC_RELAXED);
+    __atomic_add_fetch(&g_launches, 2, __ATOMIC_RELAXED);
+    /* the jobs' offsets are device addresses: the split's bases are zero */
+    const DSplitArgs D = split_args(NULL, NULL, base + L.slots, dec, d_dict, d_huf, o, bs, L.room, L.probe_warps);
+    launch_split(d_dict ? zxc_dbatch_split<true> : zxc_dbatch_split<false>, zxc_dbatch_split_scan,
+                 zxc_dbatch_split_final, A, D, (u32)grid_for((u32)L.Jt), n < 1024 ? n : 1024, st);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 
@@ -2102,14 +2070,11 @@ extern "C" int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_
     ds_layout(bs, n, 1, &L);
     if (L.total > scratch_size) return ZXC_ERROR_MEMORY;
     /* the largest direct table whose layout fits: L.total grows with J */
-    u32 lo = 1, hi = DS_J_MAX;
-    while (lo < hi) {
-        const u32 mid = lo + (hi - lo + 1) / 2;
-        ds_layout(bs, n, mid, &L);
-        if (L.total <= scratch_size) lo = mid;
-        else hi = mid - 1;
-    }
-    ds_layout(bs, n, lo, &L);
+    ds_layout(bs, n, (u32)largest_fit(1, DS_J_MAX, [&](u64 J) {
+                  ds_layout(bs, n, (u32)J, &L);
+                  return L.total <= scratch_size;
+              }),
+              &L);
     cudaStream_t st = (cudaStream_t)stream;
     u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
     DSeekState* S = (DSeekState*)base;

@@ -71,37 +71,40 @@ int zxg_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint3
                         const uint8_t* h_dict_huf_lens, const zxg_frame_bytes_t* fb, void* d_scratch,
                         size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
 
-/* Device-to-device decompress (zxc_b200_decompress_device).  The host passes what needs no frame bytes: the
- * dictionary (copied into the scratch), its zxc_dict_id and the dict_huf_attach verdict of its table (h_dict_huf NULL
- * unless that table is used).  Scratch for frames of at most block_size-byte blocks decoded into dst_capacity bytes
- * (0 without a device or for a dst_capacity too large to plan); ZXC_ERROR_MEMORY when the scratch holds less than
- * that for 4 KiB blocks. */
+/* The decode options of a device-resident decode, resolved on the host from zxc_decompress_opts_t: what needs no
+ * frame bytes. */
+typedef struct {
+    const void* dict;     /* NULL without a dictionary; copied into the scratch */
+    const void* dict_huf; /* its literal table, NULL unless dict_huf_attach finds it usable */
+    uint32_t dict_size;
+    uint32_t dict_id;     /* zxc_dict_id of the dictionary */
+    int huf_verdict;      /* dict_huf_attach of its table: 1 usable, 0 none, < 0 malformed */
+    int checksum_enabled;
+} zxg_dopts_t;
+
+/* Device-to-device decompress (zxc_b200_decompress_device).  Scratch for frames of at most block_size-byte blocks
+ * decoded into dst_capacity bytes (0 without a device or for a dst_capacity too large to plan); ZXC_ERROR_MEMORY when
+ * the scratch holds less than that for 4 KiB blocks. */
 size_t zxg_decompress_scratch_bytes(uint64_t dst_capacity, uint32_t block_size);
 int zxg_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
-                          const void* h_dict, uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id,
-                          int huf_verdict, int checksum_enabled, void* d_scratch, size_t scratch_size,
-                          int64_t* d_result, void* stream);
+                          const zxg_dopts_t* o, void* d_scratch, size_t scratch_size, int64_t* d_result, void* stream);
 
 /* In-place decode of a device-resident frame (zxc_b200_decompress_inplace_device; kernels in zxc_dinplace.cuh): the
- * frame of comp_size bytes lies flush-right in d_buffer[0 .. buffer_capacity) and decodes into d_buffer[0 ..).  The
- * host passes what zxg_decompress_device takes; ZXC_ERROR_MEMORY when the scratch holds less than the layout for 4 KiB
+ * frame of comp_size bytes lies flush-right in d_buffer[0 .. buffer_capacity) and decodes into d_buffer[0 ..).
+ * ZXC_ERROR_MEMORY when the scratch holds less than the layout for 4 KiB
  * blocks and the smallest window.  The scratch size for a window of `window` compressed bytes per round (0 without a
  * device or when that cannot be planned). */
 size_t zxg_decompress_inplace_scratch_bytes(uint64_t buffer_capacity, uint32_t block_size, uint64_t window);
-int zxg_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size, const void* h_dict,
-                                  uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id, int huf_verdict,
-                                  int checksum_enabled, void* d_scratch, size_t scratch_size, int64_t* d_result,
-                                  void* stream);
+int zxg_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size, const zxg_dopts_t* o,
+                                  void* d_scratch, size_t scratch_size, int64_t* d_result, void* stream);
 
 /* Many device-resident frames in one call (zxc_b200_decompress_device_batch; kernels in zxc_dbatch.cuh), with the
  * host's share of the verdicts made as for zxg_decompress_device.  Scratch for up to max_frames frames of at most
  * max_total_capacity output bytes in all and block_size-byte blocks (0 without a device or when that cannot be
  * planned); ZXC_ERROR_MEMORY when the scratch holds less than that for no output and 4 KiB blocks. */
 size_t zxg_decompress_batch_scratch_bytes(uint32_t max_frames, uint64_t max_total_capacity, uint32_t block_size);
-int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const void* h_dict,
-                                uint32_t dict_size, const void* h_dict_huf, uint32_t dict_id, int huf_verdict,
-                                int checksum_enabled, void* d_scratch, size_t scratch_size, int64_t* d_results,
-                                void* stream);
+int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const zxg_dopts_t* o,
+                                void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);
 
 /* Many device-resident buffers compressed in one call (zxc_b200_compress_device_batch; kernels in zxc_cbatch.cuh), with
  * the options checked and the shared frame bytes (file header, EOF block header) written by the host.  Scratch for up
