@@ -328,6 +328,95 @@ ZXC_EXPORT int zxc_b200_compress_device_batch(const zxc_b200_frame_t* d_frames, 
                                               const zxc_compress_opts_t* opts, void* d_scratch, size_t scratch_size,
                                               int64_t* d_results, void* stream);
 
+/* ---- the block API in HBM: zxc_compress_block / zxc_decompress_block(_safe) over a batch of frameless blocks ---- */
+/* Device scratch for one zxc_b200_compress_blocks_device call of at most max_blocks items whose src_size values add
+ * up to at most max_total_src, none above max_src_size bytes, at these options (0: a dictionary above
+ * ZXC_DICT_SIZE_MAX, no device, more than 2^30 items, more than 2^50 bytes, or max_src_size above
+ * ZXC_BLOCK_SIZE_MAX).  It is about 72 bytes per item, the dictionary's region, a pool of at most 2 x max_total_src +
+ * 586 x max_blocks bytes (each item's share, below), and one encode slot (zxc_b200_encode_scratch_size's per-warp
+ * share at block size B = zxf_block_size_ceil(max_src_size)) for each of W = min(max_blocks, max_total_src, resident
+ * encode grid) warps (at least one), rounded down to a multiple of 4 from 4 up: on an H100 (132 SMs, 4 224 warps), 2^20 items of 4 KiB at level 5
+ * take about 10.3 GB. */
+ZXC_EXPORT size_t zxc_b200_compress_blocks_device_scratch_size(uint32_t max_blocks, uint64_t max_total_src,
+                                                               uint32_t max_src_size, const zxc_compress_opts_t* opts);
+
+/* Compresses n_items independent frameless blocks on `stream`, asynchronously: d_items[i] (device memory) names item
+ * i's bytes src[0 .. src_size) and its block's room dst[0 .. dst_capacity), all in device memory.  d_results[i] (one
+ * device int64 per item) and dst[0 .. d_results[i]) become exactly what this library's zxc_compress_block returns and
+ * writes for item i on a fresh zxc_create_cctx(NULL) context with the same opts, and so what the reference's
+ * zxc_compress_block gives (a block's bytes depend on its content, level, checksum flag and dictionary only, not on
+ * opts->block_size).  opts == NULL means level 3 without checksums; the call uses level, checksum_enabled and one
+ * dictionary (dict / dict_size in HOST memory, read before the call returns, as for zxc_b200_compress_device);
+ * dict_huf and block_size are ignored, as by the host block API.
+ * Per item, in zxc_compress_block's order: ZXC_ERROR_NULL_INPUT for a NULL src or dst, src_size 0 or dst_capacity 0;
+ * ZXC_ERROR_BAD_BLOCK_SIZE for src_size above ZXC_BLOCK_SIZE_MAX; ZXC_ERROR_MEMORY by the room rule below; last
+ * ZXC_ERROR_DST_TOO_SMALL when the block does not fit dst_capacity (dst is then left untouched).
+ * Returns ZXC_OK once enqueued, or a verdict for the whole call that replaces every item's own (d_results is then not
+ * written), in this order: ZXC_ERROR_NULL_INPUT for a NULL d_items, d_results or d_scratch when n_items > 0;
+ * ZXC_ERROR_DICT_TOO_LARGE; ZXC_B200_ERROR_NO_DEVICE; ZXC_ERROR_MEMORY when scratch_size is below
+ * zxc_b200_compress_blocks_device_scratch_size(n_items, 0, 0, opts): the item records and one encode slot at 4 KiB.  n_items == 0 returns ZXC_OK after those checks and launches nothing.
+ * The scratch: past about 72 bytes per item and the dictionary comes the room.  Items that pass the checks take their
+ * share of it in index order from its start: an input copy of r256(src_size + 64) bytes and a staging slot of
+ * r256(src_size + 12) bytes (the most the encoder writes for a block: a RAW block with its checksum).  The encode
+ * slots are laid out for B, the largest zxf_block_size_ceil(src_size) among the admitted items, and counted down from
+ * the room's end.  Item i is admitted when the shares of the admitted items up to it plus one encode slot at B fit the
+ * room; from the first item that is not, it and every later item that passed the checks get ZXC_ERROR_MEMORY and
+ * nothing is written for them.  B and the room follow from scratch_size and the items alone: there is no block size
+ * to choose.  The call launches W warps (W as in the size query, for n_items), and every one whose slot fits the part
+ * of the room the admitted shares leave free runs (W for n_items items: min(n_items, resident grid)), so a scratch
+ * from zxc_b200_compress_blocks_device_scratch_size(n, T, m, opts) gives any batch of at most n items of at most T bytes
+ * in all and m bytes each no ZXC_ERROR_MEMORY and that query's W warps, and a smaller one runs fewer warps (down to
+ * one: same output, slower).
+ * Nothing outside [src, src + src_size) of each item is read, whatever its alignment; nothing outside the union of the
+ * dst[0 .. dst_capacity), the scratch and d_results is written, and overlapping outputs get unspecified bytes.  There
+ * is no host synchronisation and no allocation without a dictionary, and the call may then be captured in a CUDA
+ * graph; d_items, the items' bytes and d_results may change between replays.  Kernel launches per call
+ * (zxc_b200_launch_count): 5 whatever the items (checks and shares, scan, gather, encode, fit and copy-out), plus one
+ * dictionary-seeding kernel with a dictionary. */
+ZXC_EXPORT int zxc_b200_compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items,
+                                               const zxc_compress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                                               int64_t* d_results, void* stream);
+
+/* Device scratch for one zxc_b200_decompress_blocks_device call of at most max_blocks items, none with a dst_capacity
+ * above max_dst_capacity (0: no device, or more than 2^30 items).  B = zxf_block_size_ceil(max_dst_capacity); it
+ * holds, per item, 16 bytes and one job and status word in each of the k x 2 launch slots (k block sizes from 4 KiB up
+ * to B, 28 bytes each), the dictionary's region (ZXC_DICT_SIZE_MAX) and the decode kernels' per-warp scratch at B for
+ * max_blocks jobs (one warp per job up to the resident grid): on an H100, 2^20 items at 4 KiB take about 160 MiB. */
+ZXC_EXPORT size_t zxc_b200_decompress_blocks_device_scratch_size(uint32_t max_blocks, uint64_t max_dst_capacity);
+
+/* Decompresses n_items independent frameless blocks on `stream`, asynchronously: d_items[i] (device memory) names item
+ * i's block src[0 .. src_size) and its output dst[0 .. dst_capacity), all in device memory.  d_results[i] (one device
+ * int64 per item) and dst[0 .. d_results[i]) become exactly what this library's zxc_decompress_block returns and
+ * writes for item i (zxc_decompress_block_safe when safe != 0) with the same opts: checksums verified when
+ * opts->checksum_enabled, dict / dict_size (HOST memory, one for the batch, staged as for zxc_b200_decompress_device)
+ * used as there, dict_huf ignored as there.  On a negative result the item's dst holds unspecified bytes.
+ * Per item: ZXC_ERROR_NULL_INPUT for a NULL src or dst, src_size below 8 or dst_capacity 0; ZXC_ERROR_BAD_BLOCK_SIZE
+ * for dst_capacity above ZXC_BLOCK_SIZE_MAX + 2112 (safe: above ZXC_BLOCK_SIZE_MAX); ZXC_ERROR_MEMORY when
+ * zxf_block_size_ceil(dst_capacity) is above the block size B the scratch was sized for; then the block's own verdict
+ * from the decode kernels of zxc_b200_decode_blocks, run on the job {src, dst, min(src_size, 2^32 - 1), dst_capacity}
+ * at block size zxf_block_size_ceil(dst_capacity), exactly as zxc_decompress_block builds it.
+ * Returns ZXC_OK once enqueued, or a verdict for the whole call that replaces every item's own (d_results is then not
+ * written): ZXC_ERROR_NULL_INPUT for a NULL d_items, d_results or d_scratch when n_items > 0;
+ * ZXC_ERROR_DICT_TOO_LARGE; ZXC_B200_ERROR_NO_DEVICE; ZXC_ERROR_MEMORY when scratch_size is below
+ * zxc_b200_decompress_blocks_device_scratch_size(n_items, 4096).  n_items == 0 returns ZXC_OK after those checks and
+ * launches nothing.  B is the largest block size whose layout for n_items items fits scratch_size, so a scratch from
+ * zxc_b200_decompress_blocks_device_scratch_size(n, C) gives every batch of at most n items of capacity at most C a B
+ * of at least zxf_block_size_ceil(C), and the job table always holds every item.
+ * Reads: the decode kernels copy literal runs with aligned 4-byte loads that reach at most 6 bytes before and 8 bytes
+ * past a run.  A run starts behind the 8-byte block header, and in a GLO or GHI block the encoder's format keeps every
+ * literal at least 32 bytes before the payload's end, but a RAW block's run ends where the payload ends: without a
+ * checksum that is src + src_size.  So keep 8 readable bytes behind src + src_size (blocks packed back to back in one
+ * allocation have them, but for the last); nothing before src is read.  d_items and d_results must not overlap the
+ * outputs.  Nothing outside the union of the dst[0 .. dst_capacity), the scratch and d_results is written.  There is no
+ * host synchronisation and no allocation without a dictionary, and the call may then be captured in a CUDA graph;
+ * d_items, the blocks' bytes and d_results may change between replays.  Kernel launches per call
+ * (zxc_b200_launch_count): 4 + k x (2 + c) whatever the items, k the number of block sizes from 4 KiB up to B and c = 1
+ * when opts->checksum_enabled, else 0 (plan: 3; per block size the decode kernels' lean and general instance, and the
+ * verifying instance with checksums; finish: 1). */
+ZXC_EXPORT int zxc_b200_decompress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items,
+                                                 const zxc_decompress_opts_t* opts, int safe, void* d_scratch,
+                                                 size_t scratch_size, int64_t* d_results, void* stream);
+
 /* ---- random access into a seekable frame in HBM: the device twin of zxc_seekable_open +
  *      zxc_seekable_decompress_range, for many ranges per call ---- */
 typedef struct zxc_b200_seekable_device_s zxc_b200_seekable_device;

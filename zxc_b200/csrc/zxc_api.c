@@ -1096,6 +1096,47 @@ int zxc_b200_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t 
     return zxg_decompress_device_batch(d_frames, n_frames, &o, d_scratch, scratch_size, d_results, stream);
 }
 
+/* ---- the block API in HBM: zxc_compress_block / zxc_decompress_block(_safe) over a batch ---- */
+size_t zxc_b200_compress_blocks_device_scratch_size(uint32_t max_blocks, uint64_t max_total_src, uint32_t max_src_size,
+                                                    const zxc_compress_opts_t* opts) {
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    if (dict_size > ZXC_DICT_SIZE_MAX) return 0;
+    return zxg_compress_blocks_scratch_bytes(max_blocks, max_total_src, max_src_size, level_clamp(opts ? opts->level : 0),
+                                             (uint32_t)dict_size);
+}
+
+/* The host decides what needs no descriptor; the device makes zxc_compress_block's per-item checks and the rest and
+ * writes them to d_results (zxc_blocks.cuh).  The options resolve as on a fresh zxc_create_cctx(NULL) context. */
+int zxc_b200_compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, const zxc_compress_opts_t* opts,
+                                    void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+    if (n_items > 0 && (!d_items || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
+    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
+    const int irc = zxg_init();
+    if (irc != ZXC_OK || n_items == 0) return irc;
+    return zxg_compress_blocks_device(d_items, n_items, level_clamp(opts ? opts->level : 0),
+                                      opts ? opts->checksum_enabled : 0, dict, (uint32_t)dict_size, d_scratch,
+                                      scratch_size, d_results, stream);
+}
+
+size_t zxc_b200_decompress_blocks_device_scratch_size(uint32_t max_blocks, uint64_t max_dst_capacity) {
+    return zxg_decompress_blocks_scratch_bytes(max_blocks, max_dst_capacity);
+}
+
+int zxc_b200_decompress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items,
+                                      const zxc_decompress_opts_t* opts, int safe, void* d_scratch,
+                                      size_t scratch_size, int64_t* d_results, void* stream) {
+    if (n_items > 0 && (!d_items || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
+    zxg_dopts_t o;
+    const int orc = device_dopts(opts, &o);
+    if (orc != ZXC_OK) return orc;
+    o.dict_huf = NULL; /* the block API attaches no literal table (decode_one_block) */
+    const int irc = zxg_init();
+    if (irc != ZXC_OK || n_items == 0) return irc;
+    return zxg_decompress_blocks_device(d_items, n_items, &o, safe, d_scratch, scratch_size, d_results, stream);
+}
+
 int64_t zxc_compress_cctx(zxc_cctx* cctx, const void* src, size_t src_size, void* dst, size_t dst_capacity,
                           const zxc_compress_opts_t* opts) {
     if (!cctx) return ZXC_ERROR_NULL_INPUT;

@@ -30,6 +30,7 @@
 #include "zxc_dplan.cuh"
 #include "zxc_dinplace.cuh"
 #include "zxc_dseek.cuh"
+#include "zxc_blocks.cuh"
 #include "zxc_train.cuh"
 
 /* ========================================================================= */
@@ -1975,6 +1976,189 @@ extern "C" int zxg_decompress_device_batch(const zxc_b200_frame_t* d_frames, uin
     const DSplitArgs D = split_args(NULL, NULL, base + L.slots, dec, d_dict, d_huf, o, bs, L.room, L.probe_warps);
     launch_split(d_dict ? zxc_dbatch_split<true> : zxc_dbatch_split<false>, zxc_dbatch_split_scan,
                  zxc_dbatch_split_final, A, D, (u32)grid_for((u32)L.Jt), n < 1024 ? n : 1024, st);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* the block API in HBM (zxc_b200_compress_blocks_device,                    */
+/* zxc_b200_decompress_blocks_device: kernels in zxc_blocks.cuh)             */
+/* ------------------------------------------------------------------------- */
+/* Compress scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned):
+ *   BlocksCState | items (n x BlocksCItem) | tile sums (2 per tile) | dictionary region (with a dictionary) | room
+ * The room holds the pool from its start and the encode slots from its end (zxc_blocks.cuh). */
+static size_t bk_clayout(u32 n, u32 dict_size, size_t* items, size_t* tiles, size_t* dict) {
+    const size_t n_tiles = ((size_t)n + ASM_TILE - 1) / ASM_TILE;
+    size_t o = BK_STATE_BYTES;
+    *items = o;
+    o += r256((size_t)n * sizeof(BlocksCItem));
+    *tiles = o;
+    o += r256(n_tiles * 16);
+    *dict = o;
+    if (dict_size) o += r256(enc_dict_bytes(dict_size));
+    return o; /* the room's offset */
+}
+
+/* encode warps of a call over n items: one per item up to the resident grid, whole CTAs from ENC_WARPS_PER_CTA up */
+static u32 bk_warps(u32 n) {
+    const u32 resident = (u32)(g_sm_count > 0 ? g_sm_count : 132) * ENC_CTAS_PER_SM * ENC_WARPS_PER_CTA;
+    u32 W = n < resident ? n : resident;
+    if (W >= ENC_WARPS_PER_CTA) W -= W % ENC_WARPS_PER_CTA;
+    return W ? W : 1u;
+}
+
+extern "C" size_t zxg_compress_blocks_scratch_bytes(uint32_t max_blocks, uint64_t max_total_src, uint32_t max_src_size,
+                                                    int level, uint32_t dict_size) {
+    if (zxg_init() != ZXC_OK || max_blocks > CB_FRAMES_MAX || max_total_src > (1ull << 50) ||
+        max_src_size > ZXC_BLOCK_SIZE_MAX)
+        return 0;
+    size_t items, tiles, dict;
+    const size_t room = bk_clayout(max_blocks, dict_size, &items, &tiles, &dict);
+    /* an n-byte item's share is r256(n + 64) + r256(n + 12) <= 2 n + 586 bytes, for at most k non-empty items */
+    const u64 k = max_blocks < max_total_src ? max_blocks : max_total_src;
+    const u64 pool = r256(2 * max_total_src + 586 * k);
+    /* no more encode slots than items that can be non-empty: a scratch for no bytes holds one, the call's minimum */
+    const size_t ws = enc_layout((u32)zxf_block_size_ceil(max_src_size), level).total;
+    const u32 W = bk_warps(k < max_blocks ? (u32)k : max_blocks);
+    return room + pool + (size_t)W * ws + 256; /* base alignment slack */
+}
+
+extern "C" int zxg_compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, int level, int checksum,
+                                          const void* h_dict, uint32_t dict_size, void* d_scratch, size_t scratch_size,
+                                          int64_t* d_results, void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    const u32 n = n_items;
+    if (n > CB_FRAMES_MAX) return ZXC_ERROR_MEMORY;
+    const u32 dsz = h_dict && dict_size ? dict_size : 0;
+    size_t items, tiles, dict;
+    const size_t room = bk_clayout(n, dsz, &items, &tiles, &dict);
+    if (scratch_size < room + enc_layout(ZXC_BLOCK_SIZE_MIN, level).total + 256) return ZXC_ERROR_MEMORY;
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    BlocksCArgs A;
+    A.items = d_items;
+    A.results = (long long*)d_results;
+    A.st = (BlocksCState*)base;
+    A.I = (BlocksCItem*)(base + items);
+    A.tiles = (unsigned long long*)(base + tiles);
+    A.room = base + room;
+    A.room_bytes = (scratch_size - 256 - room) & ~(size_t)255;
+    for (u32 c = 0; c < BK_CLASSES; c++) A.wstride[c] = enc_layout(ZXC_BLOCK_SIZE_MIN << c, level).total;
+    A.n = n;
+    A.warps = bk_warps(n);
+    EncodeParams P;
+    memset(&P, 0, sizeof P);
+    P.counter = &A.st->counter;
+    if (dsz) { /* the block API attaches no shared literal table */
+        const int rc = enc_stage_dict(P, base + dict, h_dict, dsz, level, NULL, st);
+        if (rc != ZXC_OK) return rc;
+    }
+    P.level = (u32)level;
+    P.checksum = checksum ? 1u : 0u;
+    P.dict_size = dsz;
+    const u32 sms = (u32)(g_sm_count > 0 ? g_sm_count : 132);
+    const u32 n_tiles = (n + ASM_TILE - 1) / ASM_TILE;
+    const u32 by_warp = (n + BK_THREADS / 32 - 1) / (BK_THREADS / 32);
+    const u32 wgrid = by_warp < sms * 16 ? by_warp : sms * 16;
+    zxc_blocks_ctiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_blocks_cscan<<<1, 1, 0, st>>>(A);
+    zxc_blocks_cgather<<<wgrid, BK_THREADS, 0, st>>>(A);
+    const u32 grid = A.warps >= ENC_WARPS_PER_CTA ? A.warps / ENC_WARPS_PER_CTA : 1u;
+    const u32 threads = A.warps >= ENC_WARPS_PER_CTA ? ENC_CTA_THREADS : 32u * A.warps;
+    if (level >= 6) zxc_blocks_encode<true><<<grid, threads, 0, st>>>(P, A);
+    else zxc_blocks_encode<false><<<grid, threads, 0, st>>>(P, A);
+    zxc_blocks_cfinish<<<wgrid, BK_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 5, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* Decompress scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned):
+ *   DBatchState | dictionary region | items (n x BlocksDItem) | slot tile sums (n_slots per tile) | slot windows
+ *   (n_slots x n jobs) | slot status (n_slots x n x i32) | decode scratch for n jobs at B
+ * n_slots = 2 per block size from 4 KiB up to B (checksum verification off / on, dp_slot's numbering). */
+struct BlocksDLayout {
+    size_t dict, items, stiles, jobs, status, dec, dec_bytes, total;
+    u32 n_slots;
+};
+static void bk_dlayout(u32 n, u32 bs, BlocksDLayout* L) {
+    const size_t n_tiles = ((size_t)n + ASM_TILE - 1) / ASM_TILE;
+    L->n_slots = ((u32)__builtin_ctz(bs) - ZXC_BLOCK_SIZE_MIN_LOG2 + 1) * 2;
+    size_t o = DB_STATE_BYTES;
+    L->dict = o;
+    o += r256((size_t)ZXC_DICT_SIZE_MAX);
+    L->items = o;
+    o += r256((size_t)n * sizeof(BlocksDItem));
+    L->stiles = o;
+    o += r256(n_tiles * L->n_slots * 8);
+    L->jobs = o;
+    o += r256((size_t)L->n_slots * n * sizeof(zxc_b200_job_t));
+    L->status = o;
+    o += r256((size_t)L->n_slots * n * 4);
+    L->dec = o;
+    L->dec_bytes = launch_scratch_bytes(n ? n : 1, bs);
+    L->total = o + L->dec_bytes + 256; /* base alignment slack */
+}
+
+extern "C" size_t zxg_decompress_blocks_scratch_bytes(uint32_t max_blocks, uint64_t max_dst_capacity) {
+    if (zxg_init() != ZXC_OK || max_blocks > DB_FRAMES_MAX) return 0;
+    BlocksDLayout L;
+    bk_dlayout(max_blocks, (u32)zxf_block_size_ceil(max_dst_capacity), &L);
+    return L.total;
+}
+
+extern "C" int zxg_decompress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, const zxg_dopts_t* o,
+                                            int safe, void* d_scratch, size_t scratch_size, int64_t* d_results,
+                                            void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    const u32 n = n_items;
+    if (n > DB_FRAMES_MAX) return ZXC_ERROR_MEMORY;
+    BlocksDLayout L;
+    const u32 bs = largest_block_size([&](u32 b) {
+        bk_dlayout(n, b, &L);
+        return L.total <= scratch_size;
+    });
+    if (!bs) return ZXC_ERROR_MEMORY;
+    bk_dlayout(n, bs, &L);
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    u8 *d_dict, *d_huf;
+    const int drc = dec_stage_dict(base + L.dict, o, st, &d_dict, &d_huf);
+    if (drc != ZXC_OK) return drc;
+    DBatchState* S = (DBatchState*)base;
+    BlocksDArgs A;
+    A.items = d_items;
+    A.results = (long long*)d_results;
+    A.st = S;
+    A.I = (BlocksDItem*)(base + L.items);
+    A.stiles = (unsigned long long*)(base + L.stiles);
+    A.jobs = (zxc_b200_job_t*)(base + L.jobs);
+    A.status = (i32*)(base + L.status);
+    A.cap_max = safe ? (u64)ZXC_BLOCK_SIZE_MAX : (u64)ZXC_BLOCK_SIZE_MAX + ZXF_TAIL_PAD;
+    A.n = n;
+    A.n_slots = L.n_slots;
+    A.bs = bs;
+    A.verify = o->checksum_enabled ? 1u : 0u;
+    /* zxc_dbatch_slots reads the state, the slot tile sums and the window size n */
+    DBatchArgs D;
+    memset(&D, 0, sizeof D);
+    D.st = S;
+    D.stiles = A.stiles;
+    D.Jt = n;
+    D.n = n;
+    D.n_slots = L.n_slots;
+    const u32 per_item = (n + BK_THREADS - 1) / BK_THREADS;
+    zxc_blocks_dcount<<<(n + ASM_TILE - 1) / ASM_TILE, ASM_THREADS, 0, st>>>(A);
+    zxc_dbatch_slots<<<1, ASM_SCAN_THREADS, 0, st>>>(D);
+    zxc_blocks_dplace<<<per_item, BK_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 3, __ATOMIC_RELAXED);
+    if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    /* the jobs' offsets are device addresses: the decode's bases are zero */
+    const int rc = launch_slot_decodes(NULL, NULL, A.jobs, A.status, n, n, S->ctr, d_dict, NULL, o, base + L.dec,
+                                       L.dec_bytes, bs, st);
+    if (rc != ZXC_OK) return rc;
+    zxc_blocks_dfinish<<<per_item, BK_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 

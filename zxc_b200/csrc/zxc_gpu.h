@@ -117,6 +117,18 @@ int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frame
                               const uint8_t* h_dict_huf_lens, const uint8_t* header, const uint8_t* eof,
                               void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);
 
+/* The block API in HBM (zxc_b200_compress_blocks_device, zxc_b200_decompress_blocks_device; kernels in
+ * zxc_blocks.cuh), with the options checked by the host.  Scratch sizes (0 without a device or when that cannot be
+ * planned); ZXC_ERROR_MEMORY when the scratch holds less than the call's minimum. */
+size_t zxg_compress_blocks_scratch_bytes(uint32_t max_blocks, uint64_t max_total_src, uint32_t max_src_size, int level,
+                                         uint32_t dict_size);
+int zxg_compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, int level, int checksum,
+                               const void* h_dict, uint32_t dict_size, void* d_scratch, size_t scratch_size,
+                               int64_t* d_results, void* stream);
+size_t zxg_decompress_blocks_scratch_bytes(uint32_t max_blocks, uint64_t max_dst_capacity);
+int zxg_decompress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, const zxg_dopts_t* o, int safe,
+                                 void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);
+
 /* Device-resident seekable frames (zxc_dseek.c; kernels in zxc_dseek.cuh).  What a range call needs of its handle. */
 typedef struct {
     const void* d_src;

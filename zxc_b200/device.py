@@ -8,8 +8,9 @@ a seekable frame in HBM with zxc_b200_seekable_device_decompress_ranges.  ``deco
 in one zxc_b200_decompress_device_batch call, and ``compress_frames`` compresses many tensors into one frame each in
 one zxc_b200_compress_device_batch call.  ``decompress_inplace`` decodes a frame that lies flush-right in a CUDA buffer
 into the same buffer with zxc_b200_decompress_inplace_device, and ``load_frame`` uses it to bring a frame from the
-host into HBM and expand it there with no second buffer.  Kept apart from ``zxc_b200`` so that importing the package
-does not import torch.
+host into HBM and expand it there with no second buffer.  ``compress_blocks`` and ``decompress_blocks`` are the block
+API in HBM: many frameless blocks per zxc_b200_compress_blocks_device / zxc_b200_decompress_blocks_device call.  Kept
+apart from ``zxc_b200`` so that importing the package does not import torch.
 """
 import ctypes as C
 import warnings
@@ -507,6 +508,142 @@ def compress_frames(srcs, *, level=0, block_size=0, checksum=False, seekable=Fal
             if rc != 0:
                 raise ZxcError(rc, "zxc_b200_compress_device_batch")
     return out, results
+
+
+lib.zxc_compress_block_bound.restype = C.c_uint64
+lib.zxc_compress_block_bound.argtypes = [C.c_size_t]
+lib.zxc_b200_compress_blocks_device_scratch_size.restype = C.c_size_t
+lib.zxc_b200_compress_blocks_device_scratch_size.argtypes = [C.c_uint32, C.c_uint64, C.c_uint32, C.c_void_p]
+lib.zxc_b200_compress_blocks_device.restype = C.c_int
+lib.zxc_b200_compress_blocks_device.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t,
+                                                C.c_void_p, C.c_void_p]
+lib.zxc_b200_decompress_blocks_device_scratch_size.restype = C.c_size_t
+lib.zxc_b200_decompress_blocks_device_scratch_size.argtypes = [C.c_uint32, C.c_uint64]
+lib.zxc_b200_decompress_blocks_device.restype = C.c_int
+lib.zxc_b200_decompress_blocks_device.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t,
+                                                  C.c_void_p, C.c_void_p]
+
+
+def _same_device(tensors, what):
+    tensors = list(tensors)
+    if not tensors:
+        raise ValueError(f"{what} is empty")
+    dev = tensors[0].device
+    for t in tensors:
+        if not t.is_cuda or not t.is_contiguous():
+            raise ValueError(f"every {what[:-1]} must be a contiguous CUDA tensor")
+        if t.device != dev:
+            raise ValueError(f"every {what[:-1]} must be on {dev}, not {t.device}")
+    return [t.reshape(-1).view(torch.uint8) for t in tensors], dev
+
+
+def _run_items(dev, ins, out, stream, call):
+    """Uploads the item descriptors (in, out) and runs call(desc, results, stream) on `stream` after the current
+    stream; returns the results tensor."""
+    with torch.cuda.device(dev):
+        current = torch.cuda.current_stream(dev)
+        stream = stream or current
+        if stream != current:
+            # the inputs were made (or written) on the current stream; the caller may drop them on return
+            stream.wait_stream(current)
+            for t in ins + out:
+                t.record_stream(stream)
+        with torch.cuda.stream(stream):
+            # page-locked, so the upload does not wait for the stream (the host allocator keeps it until it ran)
+            desc = torch.tensor([[s.data_ptr() if s.numel() else 0, s.numel(), d.data_ptr() if d.numel() else 0,
+                                  d.numel()] for s, d in zip(ins, out)], dtype=torch.int64)
+            desc = desc.pin_memory().to(dev, non_blocking=True)
+            results = torch.empty(len(ins), dtype=torch.int64, device=dev)
+            call(desc, results, stream)
+    return results
+
+
+def compress_blocks(srcs, *, level=0, checksum=False, dict=None, out=None, stream=None):
+    """Compress many contiguous CUDA tensors (their bytes), all on one device, into one frameless block each, in one
+    zxc_b200_compress_blocks_device call.
+
+    Returns (outs, results): results[i] (an int64 CUDA tensor) is exactly what zxc_compress_block gives input i on a
+    fresh context: its block size (the block is outs[i][:results[i]]) or a negative zxc_error_t code.  outs[i] holds
+    zxc_compress_block_bound(len) bytes by default; `out`, a list of contiguous uint8 tensors on the inputs' device,
+    one per input, takes the blocks instead.  The work runs on `stream` (default: the current stream), which first
+    waits for the current stream; nothing synchronises.  Argument errors raise ValueError before anything is enqueued;
+    a rejected call raises ZxcError.  dict is host bytes, one dictionary for the batch."""
+    srcs, dev = _same_device(srcs, "srcs")
+    if out is not None:
+        out = list(out)
+        if len(out) != len(srcs):
+            raise ValueError("out must hold one tensor per input")
+        for o in out:
+            _check_out(o, dev)
+    o = _Opts(level=level, checksum_enabled=int(bool(checksum)))
+    keep = []
+    if dict is not None:
+        d = bytes(dict)
+        keep.append(d)
+        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+    sizes = [t.numel() for t in srcs]
+    # 0 for a batch the call cannot plan (it then gives its exact code with a token scratch)
+    scratch_size = int(lib.zxc_b200_compress_blocks_device_scratch_size(len(srcs), sum(sizes),
+                                                                        min(max(sizes), 1 << 21), C.byref(o)))
+    if out is None:
+        out = [torch.empty(max(int(lib.zxc_compress_block_bound(n)), 1), dtype=torch.uint8, device=dev)
+               for n in sizes]
+
+    def call(desc, results, stream):
+        scratch = torch.empty(max(scratch_size, 1), dtype=torch.uint8, device=dev)
+        rc = lib.zxc_b200_compress_blocks_device(desc.data_ptr(), len(srcs), C.byref(o), scratch.data_ptr(),
+                                                 scratch_size, results.data_ptr(), stream.cuda_stream)
+        if rc != 0:
+            raise ZxcError(rc, "zxc_b200_compress_blocks_device")
+
+    return out, _run_items(dev, srcs, out, stream, call)
+
+
+def decompress_blocks(blocks, sizes, *, safe=False, checksum=False, dict=None, out=None, stream=None):
+    """Decode many frameless blocks, each a contiguous uint8 CUDA tensor on one device, in one
+    zxc_b200_decompress_blocks_device call.
+
+    sizes[i] is block i's output room (its dst_capacity).  Returns (outs, results): results[i] (an int64 CUDA tensor)
+    is exactly what zxc_decompress_block (zxc_decompress_block_safe with safe=True) gives block i: its decoded size
+    (the bytes are outs[i][:results[i]]) or a negative zxc_error_t code.  `out`, a list of contiguous uint8 tensors on
+    the blocks' device, one per block, takes the outputs instead (its sizes must equal sizes).  The work runs on
+    `stream` (default: the current stream), which first waits for the current stream; nothing synchronises.  Argument
+    errors raise ValueError before anything is enqueued; a rejected call raises ZxcError.  dict is host bytes."""
+    blocks, dev = _same_device(blocks, "blocks")
+    sizes = [int(c) for c in sizes]
+    if len(sizes) != len(blocks):
+        raise ValueError("sizes must hold one value per block")
+    if any(c < 0 for c in sizes):
+        raise ValueError("sizes must not be negative")
+    if out is not None:
+        out = list(out)
+        if len(out) != len(blocks):
+            raise ValueError("out must hold one tensor per block")
+        for o in out:
+            _check_out(o, dev)
+        if [o.numel() for o in out] != sizes:
+            raise ValueError("sizes differ from the sizes of out")
+    o = _DOpts(checksum_enabled=int(bool(checksum)))
+    keep = []
+    if dict is not None:
+        d = bytes(dict)
+        keep.append(d)
+        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+    scratch_size = int(lib.zxc_b200_decompress_blocks_device_scratch_size(len(blocks), max(sizes)))
+    if scratch_size == 0:
+        raise ValueError("zxc_b200_decompress_blocks_device_scratch_size: too many blocks, or no device")
+    if out is None:
+        out = [torch.empty(max(c, 1), dtype=torch.uint8, device=dev)[:c] for c in sizes]
+
+    def call(desc, results, stream):
+        scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
+        rc = lib.zxc_b200_decompress_blocks_device(desc.data_ptr(), len(blocks), C.byref(o), int(bool(safe)),
+                                                   scratch.data_ptr(), scratch_size, results.data_ptr(),
+                                                   stream.cuda_stream)
+        if rc != 0:
+            raise ZxcError(rc, "zxc_b200_decompress_blocks_device")
+
+    return out, _run_items(dev, blocks, out, stream, call)
 
 
 lib.zxc_b200_seekable_device_open.restype = C.c_void_p
