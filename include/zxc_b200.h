@@ -23,6 +23,7 @@
 
 #include "zxc_export.h"
 #include "zxc_opts.h"
+#include "zxc_pstream.h"
 
 #ifdef __cplusplus
 extern "C" {
@@ -489,6 +490,54 @@ ZXC_EXPORT int zxc_b200_seekable_device_decompress_ranges(zxc_b200_seekable_devi
                                                           void* d_dst, uint64_t dst_capacity, void* d_scratch,
                                                           size_t scratch_size, int64_t* d_results, void* stream);
 ZXC_EXPORT void zxc_b200_seekable_device_free(zxc_b200_seekable_device* h);
+
+/* ---- push streaming in HBM: the device twins of zxc_cstream_* / zxc_dstream_* (include/zxc_pstream.h) ---- */
+typedef struct zxc_b200_cstream_device_s zxc_b200_cstream_device;
+typedef struct zxc_b200_dstream_device_s zxc_b200_dstream_device;
+
+/* Streams whose chunks live in device memory: in->src and out->dst are device pointers on the handle's device (any
+ * alignment); the pos / size fields are host values, as for the host streams.
+ * Call for call identical to the reference: fed the same chunks and out capacities in the same order as the
+ * reference's zxc_cstream_* / zxc_dstream_*, every call gives the same return value, in->pos and out->pos, the same
+ * bytes in out->dst[0 .. out->pos), and the same _finished result and _in_size / _out_size hints.  Bytes past out->pos
+ * are unspecified.  The compressed stream is zxc_compress's non-seekable frame.
+ * Creation follows zxc_cstream_create / zxc_dstream_create: dictionary options give NULL, so does a bad block_size;
+ * level 0 means the default level and other levels are clamped; seekable, n_threads and the progress callback are
+ * ignored.  NULL also when there is no device or an allocation fails.  The handle is bound to the CUDA device current
+ * at creation; calls switch to it and back.
+ * Synchronous and ordered on `stream` (a cudaStream_t, NULL = legacy default stream): a call's work follows what is
+ * already enqueued on `stream` (a chunk a kernel just wrote there is seen), and the call returns once all its work is
+ * complete: the caller may then overwrite `in` and read `out` without waiting.  Not capturable in a CUDA graph.  The
+ * handle owns device buffers, grown to the largest batch a call has used and freed by _free.  Errors are sticky, as in
+ * the reference.  One handle must not be used by two threads at once; separate handles may run on separate streams.
+ * Reads: nothing outside in->src[in->pos .. in->size) is read.  Writes: nothing outside out->dst[0 .. out->size) and
+ * the handle's own memory is written; `in` is not written.
+ * Work per call (DESIGN.md section 7l).  Blocks go in batches of at most 64 MiB of decoded bytes, sized from the out
+ * room as on the host streams.
+ *   cstream, per batch: 3 kernel launches (zxc_b200_launch_count): encode, trailers, and the gather into `out`, plus
+ *     one gather before the batch when bytes were drained ahead of it in the call (the file header, a held block);
+ *     and 1 host synchronisation (the block sizes and trailers come back in one copy).
+ *   dstream, per batch: 4 launches: the header walk, the decode kernels' lean and general instance, and the gather;
+ *     3 when checksums are verified (opts->checksum_enabled and a frame with checksums), where the verifying instance
+ *     alone replaces the pair; and 2 host synchronisations (the walk's result in one copy, the decode statuses in
+ *     one copy).
+ *   Either: at most a few small copies per call for bytes cut by a chunk's end (file header, a block header, the
+ *   footer) and one synchronisation at the end.  None of this grows with the number of blocks in a batch. */
+ZXC_EXPORT zxc_b200_cstream_device* zxc_b200_cstream_device_create(const zxc_compress_opts_t* opts);
+ZXC_EXPORT int64_t zxc_b200_cstream_device_compress(zxc_b200_cstream_device* cs, zxc_outbuf_t* out, zxc_inbuf_t* in,
+                                                    void* stream);
+ZXC_EXPORT int64_t zxc_b200_cstream_device_end(zxc_b200_cstream_device* cs, zxc_outbuf_t* out, void* stream);
+ZXC_EXPORT size_t zxc_b200_cstream_device_in_size(const zxc_b200_cstream_device* cs);
+ZXC_EXPORT size_t zxc_b200_cstream_device_out_size(const zxc_b200_cstream_device* cs);
+ZXC_EXPORT void zxc_b200_cstream_device_free(zxc_b200_cstream_device* cs);
+
+ZXC_EXPORT zxc_b200_dstream_device* zxc_b200_dstream_device_create(const zxc_decompress_opts_t* opts);
+ZXC_EXPORT int64_t zxc_b200_dstream_device_decompress(zxc_b200_dstream_device* ds, zxc_outbuf_t* out,
+                                                      zxc_inbuf_t* in, void* stream);
+ZXC_EXPORT int zxc_b200_dstream_device_finished(const zxc_b200_dstream_device* ds);
+ZXC_EXPORT size_t zxc_b200_dstream_device_in_size(const zxc_b200_dstream_device* ds);
+ZXC_EXPORT size_t zxc_b200_dstream_device_out_size(const zxc_b200_dstream_device* ds);
+ZXC_EXPORT void zxc_b200_dstream_device_free(zxc_b200_dstream_device* ds);
 
 /* Kernels launched by this library since load (for bench.py's gpu_launches). */
 ZXC_EXPORT uint64_t zxc_b200_launch_count(void);

@@ -31,6 +31,7 @@
 #include "zxc_dinplace.cuh"
 #include "zxc_dseek.cuh"
 #include "zxc_blocks.cuh"
+#include "zxc_pstream_device.cuh"
 #include "zxc_train.cuh"
 
 /* ========================================================================= */
@@ -2160,6 +2161,114 @@ extern "C" int zxg_decompress_blocks_device(const zxc_b200_frame_t* d_items, uin
     zxc_blocks_dfinish<<<per_item, BK_THREADS, 0, st>>>(A);
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* push streams in HBM (zxc_b200_cstream_device / _dstream_device:           */
+/* zxc_pstream.c drives these, kernels in zxc_pstream_device.cuh)            */
+/* ------------------------------------------------------------------------- */
+static int ps_cuda(cudaError_t e) {
+    if (e == cudaSuccess) return ZXC_OK;
+    fprintf(stderr, "libzxc (CUDA build): device stream step failed: %s\n", cudaGetErrorString(e));
+    cudaGetLastError();
+    return ZXC_B200_ERROR_CUDA;
+}
+
+extern "C" int zxg_d2d_async(void* d_dst, const void* d_src, size_t bytes, void* stream) {
+    if (bytes == 0) return ZXC_OK;
+    return ps_cuda(cudaMemcpyAsync(d_dst, d_src, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+}
+
+extern "C" int zxg_h2d_async(void* d_dst, const void* h_src, size_t bytes, void* stream) {
+    if (bytes == 0) return ZXC_OK;
+    return ps_cuda(cudaMemcpyAsync(d_dst, h_src, bytes, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+}
+
+extern "C" int zxg_memset_async(void* d_dst, int v, size_t bytes, void* stream) {
+    if (bytes == 0) return ZXC_OK;
+    return ps_cuda(cudaMemsetAsync(d_dst, v, bytes, (cudaStream_t)stream));
+}
+
+extern "C" void* zxg_host_alloc(size_t bytes) {
+    void* h = NULL;
+    if (cudaMallocHost(&h, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return NULL;
+    }
+    return h;
+}
+
+extern "C" void zxg_host_free(void* h) {
+    if (h) cudaFreeHost(h);
+}
+
+extern "C" int zxg_stream_sync(void* stream) { return ps_cuda(cudaStreamSynchronize((cudaStream_t)stream)); }
+
+extern "C" int zxg_ps_walk(const void* d_src, uint64_t size, uint32_t max_blocks, uint64_t bound, int has_checksum,
+                           zxg_psblk_t* d_out, zxg_psblk_t* h_out, uint32_t* n_out, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    u32* d_n = (u32*)(d_out + max_blocks + 1);
+    zxc_ps_walk<<<1, 32, 0, st>>>((const u8*)d_src, size, max_blocks, bound, has_checksum ? 1u : 0u, d_out, d_n);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    /* the entries and the count are one region: one copy, one synchronisation */
+    const size_t bytes = ((size_t)max_blocks + 1) * sizeof(zxg_psblk_t) + sizeof(u32);
+    int rc = ps_cuda(cudaGetLastError());
+    if (rc == ZXC_OK) rc = ps_cuda(cudaMemcpyAsync(h_out, d_out, bytes, cudaMemcpyDeviceToHost, st));
+    if (rc == ZXC_OK) rc = ps_cuda(cudaStreamSynchronize(st));
+    if (rc == ZXC_OK) memcpy(n_out, (const u8*)h_out + bytes - sizeof(u32), sizeof(u32));
+    return rc;
+}
+
+extern "C" size_t zxg_ps_decode_scratch_bytes(uint32_t n_jobs, uint32_t block_size) {
+    return launch_scratch_bytes(n_jobs, block_size);
+}
+
+extern "C" size_t zxg_ps_encode_scratch_bytes(uint32_t n_blocks, uint32_t block_size, int level) {
+    return (size_t)enc_full_warps(n_blocks) * enc_layout(block_size, level).total;
+}
+
+extern "C" uint32_t zxg_ps_stage_stride(uint32_t block_size) { return enc_staging_stride(block_size); }
+
+extern "C" int zxg_ps_decode(const zxc_b200_job_t* h_jobs, uint32_t n, zxc_b200_job_t* d_jobs, int32_t* d_status,
+                             void* d_dst, void* d_scratch, size_t scratch_size, unsigned long long* d_counter,
+                             uint32_t block_size, int verify, int32_t* h_status, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = ps_cuda(cudaMemcpyAsync(d_jobs, h_jobs, (size_t)n * sizeof(zxc_b200_job_t), cudaMemcpyHostToDevice, st));
+    /* the jobs' offsets are device addresses: the decode's source base is zero */
+    if (rc == ZXC_OK)
+        rc = launch_decode(NULL, d_dst, d_jobs, n, d_status, NULL, 0, NULL, d_scratch, scratch_size, block_size, verify,
+                           d_counter, st, 0);
+    if (rc == ZXC_OK) rc = ps_cuda(cudaMemcpyAsync(h_status, d_status, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    if (rc == ZXC_OK) rc = ps_cuda(cudaStreamSynchronize(st));
+    return rc;
+}
+
+extern "C" int zxg_ps_encode(const void* d_src, uint64_t src_size, uint32_t block_size, int level, int checksum,
+                             uint32_t n_blocks, void* d_stage, uint32_t* d_st, void* d_scratch,
+                             unsigned long long* d_counter, uint32_t* h_st, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    const EncLaunch E = {(const u8*)d_src, src_size, block_size, n_blocks, level, checksum, (u8*)d_stage, d_st,
+                         (u8*)d_scratch, enc_full_warps(n_blocks), d_counter, NULL, NULL, 0, NULL};
+    int rc = launch_encode(E, st);
+    if (rc != ZXC_OK) return rc;
+    zxc_ps_trailers<<<(n_blocks + 255) / 256, 256, 0, st>>>((const u8*)d_stage, enc_staging_stride(block_size), d_st,
+                                                            d_st + n_blocks, n_blocks);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    rc = ps_cuda(cudaGetLastError());
+    if (rc == ZXC_OK) rc = ps_cuda(cudaMemcpyAsync(h_st, d_st, (size_t)n_blocks * 8, cudaMemcpyDeviceToHost, st));
+    if (rc == ZXC_OK) rc = ps_cuda(cudaStreamSynchronize(st));
+    return rc;
+}
+
+extern "C" int zxg_ps_gather(const zxg_psseg_t* h_segs, uint32_t n, zxg_psseg_t* d_segs, void* stream) {
+    if (n == 0) return ZXC_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    int rc = ps_cuda(cudaMemcpyAsync(d_segs, h_segs, (size_t)n * sizeof *h_segs, cudaMemcpyHostToDevice, st));
+    if (rc != ZXC_OK) return rc;
+    const u32 gmax = (u32)(g_sm_count > 0 ? g_sm_count : 132) * 8u;
+    zxc_ps_gather<<<n < gmax ? n : gmax, 256, 0, st>>>(d_segs, n);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return ps_cuda(cudaGetLastError());
 }
 
 /* ------------------------------------------------------------------------- */

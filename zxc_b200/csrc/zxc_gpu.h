@@ -150,6 +150,47 @@ size_t zxg_dseek_scratch_bytes(uint32_t block_size, uint32_t n_ranges, uint64_t 
 int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_ranges, uint32_t n_ranges, void* d_dst,
                      uint64_t dst_capacity, void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);
 
+/* Push streams in HBM (zxc_b200_cstream_device / _dstream_device: zxc_pstream.c; kernels in zxc_pstream_device.cuh).
+ * Every call enqueues on `stream`; the ones that return host values synchronise it. */
+typedef struct {
+    uint64_t off;     /* the header's offset from the walk's start */
+    uint64_t hdr;     /* its 8 bytes, little-endian */
+    uint32_t len;     /* on-disk length of a data block whole in the chunk; 0 for the header the walk stopped at */
+    uint32_t trailer; /* the block's checksum trailer (0 without checksums) */
+} zxg_psblk_t;
+typedef struct {
+    uint64_t src, dst, len; /* device addresses; len <= ZXG_PS_PIECE */
+} zxg_psseg_t;
+#define ZXG_PS_PIECE ((uint64_t)64 << 10)
+/* Walks block headers from d_src (size bytes) for at most max_blocks whole data blocks, plus the header it stopped at:
+ * h_out (max_blocks + 1 entries) and *n_out, through d_out (as large) and d_n in one copy. */
+int zxg_ps_walk(const void* d_src, uint64_t size, uint32_t max_blocks, uint64_t bound, int has_checksum,
+                zxg_psblk_t* d_out, zxg_psblk_t* h_out, uint32_t* n_out, void* stream);
+/* Device bytes of one batch: the decode scratch for n_jobs jobs; the encode's per-warp scratch and its staging stride. */
+size_t zxg_ps_decode_scratch_bytes(uint32_t n_jobs, uint32_t block_size);
+size_t zxg_ps_encode_scratch_bytes(uint32_t n_blocks, uint32_t block_size, int level);
+uint32_t zxg_ps_stage_stride(uint32_t block_size);
+/* Decodes n jobs (src_off: device addresses; dst_off: offsets into d_dst) with the jobs and statuses at d_jobs /
+ * d_status and the three work counters at d_counter; h_status gets the n statuses. */
+int zxg_ps_decode(const zxc_b200_job_t* h_jobs, uint32_t n, zxc_b200_job_t* d_jobs, int32_t* d_status, void* d_dst,
+                  void* d_scratch, size_t scratch_size, unsigned long long* d_counter, uint32_t block_size, int verify,
+                  int32_t* h_status, void* stream);
+/* Encodes n_blocks blocks of d_src (16-byte aligned, 64 zero bytes behind src_size) into staging slots of
+ * zxg_ps_stage_stride(block_size) bytes at d_stage; h_st gets the n sizes, then the n trailers (d_st as large). */
+int zxg_ps_encode(const void* d_src, uint64_t src_size, uint32_t block_size, int level, int checksum, uint32_t n_blocks,
+                  void* d_stage, uint32_t* d_st, void* d_scratch, unsigned long long* d_counter, uint32_t* h_st,
+                  void* stream);
+/* Copies the n pieces at h_segs to d_segs (n entries) and gathers them in one launch. */
+int zxg_ps_gather(const zxg_psseg_t* h_segs, uint32_t n, zxg_psseg_t* d_segs, void* stream);
+/* Stream-ordered copies, not waited for (a pageable host source has been read when they return). */
+int zxg_d2d_async(void* d_dst, const void* d_src, size_t bytes, void* stream);
+int zxg_h2d_async(void* d_dst, const void* h_src, size_t bytes, void* stream);
+int zxg_memset_async(void* d_dst, int v, size_t bytes, void* stream);
+int zxg_stream_sync(void* stream);
+/* page-locked host memory (cudaMallocHost), for copies that run at full speed; NULL on failure */
+void* zxg_host_alloc(size_t bytes);
+void zxg_host_free(void* h);
+
 /* Device selection for the calling thread (multi-device fork-join in zxc_api.c): current device, device count,
  * cudaSetDevice.  zxg_acquire() hands out a context of the calling thread's current device. */
 int zxg_current_device(void);

@@ -796,3 +796,139 @@ class SeekableFrame:
         if r < 0:
             raise ZxcError(r, "zxc_b200_seekable_device_decompress_ranges")
         return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# push streaming in HBM: zxc_b200_cstream_device / zxc_b200_dstream_device with zlib's compressobj / decompressobj shape
+# ---------------------------------------------------------------------------------------------------------------------
+class _InBuf(C.Structure):  # zxc_inbuf_t (include/zxc_pstream.h)
+    _fields_ = [("src", C.c_void_p), ("size", C.c_size_t), ("pos", C.c_size_t)]
+
+
+class _OutBuf(C.Structure):  # zxc_outbuf_t
+    _fields_ = [("dst", C.c_void_p), ("size", C.c_size_t), ("pos", C.c_size_t)]
+
+
+for _k in ("c", "d"):
+    getattr(lib, f"zxc_b200_{_k}stream_device_create").restype = C.c_void_p
+    getattr(lib, f"zxc_b200_{_k}stream_device_create").argtypes = [C.c_void_p]
+    getattr(lib, f"zxc_b200_{_k}stream_device_free").restype = None
+    getattr(lib, f"zxc_b200_{_k}stream_device_free").argtypes = [C.c_void_p]
+    getattr(lib, f"zxc_b200_{_k}stream_device_out_size").restype = C.c_size_t
+    getattr(lib, f"zxc_b200_{_k}stream_device_out_size").argtypes = [C.c_void_p]
+lib.zxc_b200_cstream_device_compress.restype = C.c_int64
+lib.zxc_b200_cstream_device_compress.argtypes = [C.c_void_p, C.POINTER(_OutBuf), C.POINTER(_InBuf), C.c_void_p]
+lib.zxc_b200_cstream_device_end.restype = C.c_int64
+lib.zxc_b200_cstream_device_end.argtypes = [C.c_void_p, C.POINTER(_OutBuf), C.c_void_p]
+lib.zxc_b200_dstream_device_decompress.restype = C.c_int64
+lib.zxc_b200_dstream_device_decompress.argtypes = [C.c_void_p, C.POINTER(_OutBuf), C.POINTER(_InBuf), C.c_void_p]
+lib.zxc_b200_dstream_device_finished.restype = C.c_int
+lib.zxc_b200_dstream_device_finished.argtypes = [C.c_void_p]
+
+# out is collected in pieces of at least this size, so a large input is one call that batches all its blocks
+_STREAM_CHUNK = 64 << 20
+
+
+class _DeviceStream:
+    def __init__(self, kind, opts):
+        self._kind = kind
+        self._device = torch.device("cuda", torch.cuda.current_device())
+        with torch.cuda.device(self._device):
+            self._h = getattr(lib, f"zxc_b200_{kind}stream_device_create")(C.byref(opts))
+        if not self._h:
+            raise ValueError(f"zxc_b200_{kind}stream_device_create rejected the options (or there is no device)")
+
+    def _src(self, t):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise ValueError("data must be a CUDA tensor")
+        if not t.is_contiguous():
+            raise ValueError("data must be contiguous")
+        if t.device != self._device:
+            raise ValueError(f"data is on {t.device}, the stream on {self._device}")
+        return t.reshape(-1).view(torch.uint8)
+
+    def _run(self, step, stream):
+        """Calls step(out, stream) with fresh out buffers until it has nothing more to give; the bytes, one tensor.
+        The result owns storage of its own size: a view of a partly filled out buffer would keep all of it alive."""
+        hint = int(getattr(lib, f"zxc_b200_{self._kind}stream_device_out_size")(self._h))
+        parts = []
+        with torch.cuda.device(self._device):
+            stream = stream or torch.cuda.current_stream(self._device)
+            while True:
+                out = torch.empty(max(_STREAM_CHUNK, hint), dtype=torch.uint8, device=self._device)
+                ob = _OutBuf(out.data_ptr(), out.numel(), 0)
+                more = step(ob, stream.cuda_stream)
+                parts.append(out if ob.pos == out.numel() else out[: ob.pos].clone())
+                if not more:
+                    break
+            return parts[0] if len(parts) == 1 else torch.cat(parts)
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            getattr(lib, f"zxc_b200_{self._kind}stream_device_free")(h)
+
+
+class DeviceCompress(_DeviceStream):
+    """zxc_b200_cstream_device: CUDA tensors in, the compressed stream out as uint8 CUDA tensors.  Every call runs on
+    `stream` (default: torch's current stream of the stream's device) and returns once its work is complete."""
+
+    def __init__(self, level=0, block_size=0, checksum=False):
+        super().__init__("c", _Opts(level=level, block_size=block_size, checksum_enabled=int(bool(checksum))))
+
+    def _call(self, fn, what, *args):
+        r = fn(self._h, *args)
+        if r < 0:
+            raise ZxcError(r, what)
+        return r != 0
+
+    def compress(self, data, stream=None):
+        """Feeds data; returns the compressed bytes this made available (whole blocks, and the header first)."""
+        b = self._src(data)
+        ib = _InBuf(b.data_ptr() if b.numel() else None, b.numel(), 0)
+        return self._run(lambda ob, st: self._call(lib.zxc_b200_cstream_device_compress, "zxc_b200_cstream_device_compress",
+                                                   C.byref(ob), C.byref(ib), st), stream)
+
+    def flush(self, stream=None):
+        """Ends the stream: the last block, the EOF block and the footer.  The object is finished afterwards."""
+        return self._run(lambda ob, st: self._call(lib.zxc_b200_cstream_device_end, "zxc_b200_cstream_device_end",
+                                                   C.byref(ob), st), stream)
+
+
+class DeviceDecompress(_DeviceStream):
+    """zxc_b200_dstream_device: compressed CUDA tensors in, decoded bytes out as uint8 CUDA tensors; `eof` and
+    `unused_data` (a view of the last input, then of the inputs after the end) as for zlib's decompressobj."""
+
+    def __init__(self, checksum=False):
+        super().__init__("d", _DOpts(checksum_enabled=int(bool(checksum))))
+        self.eof = False
+        self.unused_data = torch.empty(0, dtype=torch.uint8, device=self._device)
+
+    def decompress(self, data, stream=None):
+        """Feeds compressed bytes; returns what they decode to.  Bytes after the stream's footer go to unused_data."""
+        b = self._src(data)
+        if self.eof:
+            self.unused_data = torch.cat([self.unused_data, b]) if self.unused_data.numel() else b
+            return torch.empty(0, dtype=torch.uint8, device=self._device)
+        ib = _InBuf(b.data_ptr() if b.numel() else None, b.numel(), 0)
+
+        def step(ob, st):
+            r = lib.zxc_b200_dstream_device_decompress(self._h, C.byref(ob), C.byref(ib), st)
+            if r < 0:
+                raise ZxcError(r, "zxc_b200_dstream_device_decompress")
+            if lib.zxc_b200_dstream_device_finished(self._h):
+                self.eof = True
+                self.unused_data = b[ib.pos:]
+                return False
+            return ob.pos == ob.size  # out full: more may be waiting
+        return self._run(step, stream)
+
+
+def compressobj(level=0, block_size=0, checksum=False):
+    """A push-streaming compressor for CUDA tensors on the current device (zxc_b200.stream.compressobj's shape)."""
+    return DeviceCompress(level, block_size, checksum)
+
+
+def decompressobj(checksum=False):
+    """A push-streaming decompressor for CUDA tensors on the current device (zxc_b200.stream.decompressobj's shape)."""
+    return DeviceDecompress(checksum)
