@@ -418,6 +418,80 @@ ZXC_EXPORT int zxc_b200_decompress_blocks_device(const zxc_b200_frame_t* d_items
                                                  const zxc_decompress_opts_t* opts, int safe, void* d_scratch,
                                                  size_t scratch_size, int64_t* d_results, void* stream);
 
+/* ---- prepared dictionaries in HBM: load a dictionary once, use it in every device-to-device call ---- */
+typedef struct zxc_b200_dict_device_s zxc_b200_dict_device;
+
+/* Prepares the dictionary dict[0 .. dict_size) and its optional 128-byte literal table dict_huf (HOST memory, pageable
+ * or page-locked; read before the call returns, so the caller may free or overwrite them afterwards) for the
+ * _using_dict calls below.  Synchronous on `stream` (a cudaStream_t, NULL = legacy default stream): the call returns
+ * once the device copy is complete.  The handle owns one device allocation on the CUDA device current at creation, to
+ * which it is bound, of about 2 x dict_size + 520 KiB: the dictionary as the decode calls stage it (its table right
+ * behind it when the table is usable), and as the compress calls stage it (zero-padded, with the match tables that
+ * zxc_seed_kernel seeds for levels 1-2 and for levels 3-7, and the table's 256 code lengths).  Creation runs two
+ * seeding kernels.  A malformed dict_huf is not rejected here: the handle keeps the verdicts the calls would make about
+ * it, and every _using_dict call gives them where its base call does (ZXC_ERROR_CORRUPT_DATA from the frame compress
+ * calls, the device verdict of the frame decode calls).
+ * Returns NULL and sets *err (err may be NULL; ZXC_OK on success), in this order: ZXC_ERROR_NULL_INPUT for a NULL dict
+ * or dict_size 0; ZXC_ERROR_DICT_TOO_LARGE above ZXC_DICT_SIZE_MAX; ZXC_B200_ERROR_NO_DEVICE; ZXC_ERROR_MEMORY or
+ * ZXC_B200_ERROR_CUDA when the device memory cannot be allocated or filled. */
+ZXC_EXPORT zxc_b200_dict_device* zxc_b200_dict_device_create(const void* dict, size_t dict_size, const void* dict_huf,
+                                                             int* err, void* stream);
+/* zxc_dict_id(dict, dict_size, dict_huf) of the bytes the handle was created from (0 for NULL) */
+ZXC_EXPORT uint32_t zxc_b200_dict_device_id(const zxc_b200_dict_device* dd);
+/* the dictionary's content bytes (0 for NULL) */
+ZXC_EXPORT size_t zxc_b200_dict_device_size(const zxc_b200_dict_device* dd);
+/* Waits for the handle's device (calls in flight on any stream may still read the handle), then frees it.  Graphs
+ * captured with the handle are invalid afterwards.  NULL is a no-op. */
+ZXC_EXPORT void zxc_b200_dict_device_free(zxc_b200_dict_device* dd);
+
+/* The _using_dict variants.  Each takes its base call's arguments plus dd right after opts, and returns, writes to its
+ * result words and writes to its outputs exactly what the base call does when opts->dict, dict_size and dict_huf are
+ * replaced by the bytes dd was created from; with dd == NULL, what the base call does without a dictionary.  opts' own
+ * dictionary fields are ignored, so the base call's DICT_TOO_LARGE never comes.  The differences:
+ *   - No staging: the call makes no host copy, allocation or synchronisation, with or without a handle, so it may be
+ *     captured in a CUDA graph (which keeps reading the handle: free it only after the graph's last replay).
+ *   - Kernel launches (zxc_b200_launch_count): the compress variants launch no seeding kernel, so they make the base
+ *     call's dictionary-free count (6 for zxc_b200_compress_device, 1 for an empty input; 12 for _batch; 5 for
+ *     _blocks); the decode variants make the base call's count.
+ *   - Scratch: the compress variants' layouts are the base call's layouts for opts without a dictionary, so the size
+ *     queries with opts->dict = NULL give their scratch, and the pool and admission rules of _batch and _blocks are
+ *     those of a dictionary-free call (a larger scratch works too).  The results equal the base call's wherever
+ *     neither call reaches a scratch-capacity ZXC_ERROR_MEMORY.  The decode layouts are unchanged; their dictionary
+ *     region is left unused.
+ *   - A handle bound to another device than the current one gives ZXC_B200_ERROR_NO_DEVICE where the base call checks
+ *     for a device.
+ * The handle is only read by the calls: any number of calls on any streams and threads may share it. */
+ZXC_EXPORT int zxc_b200_compress_device_using_dict(const void* d_src, uint64_t src_size, void* d_dst,
+                                                   uint64_t dst_capacity, const zxc_compress_opts_t* opts,
+                                                   const zxc_b200_dict_device* dd, void* d_scratch, size_t scratch_size,
+                                                   int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
+ZXC_EXPORT int zxc_b200_compress_device_batch_using_dict(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
+                                                         const zxc_compress_opts_t* opts,
+                                                         const zxc_b200_dict_device* dd, void* d_scratch,
+                                                         size_t scratch_size, int64_t* d_results, void* stream);
+/* as zxc_b200_compress_blocks_device, the handle's literal table is not attached */
+ZXC_EXPORT int zxc_b200_compress_blocks_device_using_dict(const zxc_b200_frame_t* d_items, uint32_t n_items,
+                                                          const zxc_compress_opts_t* opts,
+                                                          const zxc_b200_dict_device* dd, void* d_scratch,
+                                                          size_t scratch_size, int64_t* d_results, void* stream);
+ZXC_EXPORT int zxc_b200_decompress_device_using_dict(const void* d_src, uint64_t src_size, void* d_dst,
+                                                     uint64_t dst_capacity, const zxc_decompress_opts_t* opts,
+                                                     const zxc_b200_dict_device* dd, void* d_scratch,
+                                                     size_t scratch_size, int64_t* d_result, void* stream);
+ZXC_EXPORT int zxc_b200_decompress_inplace_device_using_dict(void* d_buffer, uint64_t buffer_capacity,
+                                                             uint64_t comp_size, const zxc_decompress_opts_t* opts,
+                                                             const zxc_b200_dict_device* dd, void* d_scratch,
+                                                             size_t scratch_size, int64_t* d_result, void* stream);
+ZXC_EXPORT int zxc_b200_decompress_device_batch_using_dict(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
+                                                           const zxc_decompress_opts_t* opts,
+                                                           const zxc_b200_dict_device* dd, void* d_scratch,
+                                                           size_t scratch_size, int64_t* d_results, void* stream);
+/* as zxc_b200_decompress_blocks_device, the handle's literal table is not attached */
+ZXC_EXPORT int zxc_b200_decompress_blocks_device_using_dict(const zxc_b200_frame_t* d_items, uint32_t n_items,
+                                                            const zxc_decompress_opts_t* opts,
+                                                            const zxc_b200_dict_device* dd, int safe, void* d_scratch,
+                                                            size_t scratch_size, int64_t* d_results, void* stream);
+
 /* ---- random access into a seekable frame in HBM: the device twin of zxc_seekable_open +
  *      zxc_seekable_decompress_range, for many ranges per call ---- */
 typedef struct zxc_b200_seekable_device_s zxc_b200_seekable_device;

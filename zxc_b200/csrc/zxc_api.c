@@ -912,6 +912,88 @@ int64_t zxc_compress(const void* src, const size_t src_size, void* dst, const si
 }
 
 /* ---- device to device (include/zxc_b200.h) ---- */
+/* A prepared dictionary in device memory: the regions the calls would stage from its bytes, and what they would decide
+ * about its literal table. */
+struct zxc_b200_dict_device_s {
+    zxg_ddict_t g;
+    void* mem;       /* owned: zxg_ddict_bytes(size) bytes on `device` */
+    uint32_t id;     /* zxc_dict_id(dict, size, huf) */
+    int device;
+    int huf_rc;      /* unpack_dict_huf's verdict: what the frame compress calls return (ZXC_OK or CORRUPT_DATA) */
+    int huf_verdict; /* dict_huf_attach's: what the frame decode calls report on the device */
+};
+
+zxc_b200_dict_device* zxc_b200_dict_device_create(const void* dict, size_t dict_size, const void* dict_huf, int* err,
+                                                  void* stream) {
+    int rc_;
+    int* rc = err ? err : &rc_;
+    *rc = ZXC_ERROR_NULL_INPUT;
+    if (!dict || dict_size == 0) return NULL;
+    *rc = ZXC_ERROR_DICT_TOO_LARGE;
+    if (dict_size > ZXC_DICT_SIZE_MAX) return NULL;
+    *rc = zxg_init();
+    if (*rc != ZXC_OK) return NULL;
+    zxc_b200_dict_device* dd = (zxc_b200_dict_device*)calloc(1, sizeof *dd);
+    if (dd) dd->mem = zxg_dev_alloc(zxg_ddict_bytes((uint32_t)dict_size));
+    if (!dd || !dd->mem) {
+        free(dd);
+        *rc = ZXC_ERROR_MEMORY;
+        return NULL;
+    }
+    uint8_t lens[256];
+    int have_huf = 0;
+    dd->huf_rc = unpack_dict_huf((const uint8_t*)dict_huf, lens, &have_huf);
+    dd->huf_verdict = dict_huf_attach((const uint8_t*)dict_huf);
+    dd->id = zxc_dict_id(dict, dict_size, dict_huf);
+    dd->device = zxg_current_device();
+    *rc = zxg_ddict_build(dd->mem, dict, (uint32_t)dict_size, dd->huf_verdict == 1 ? dict_huf : NULL,
+                          dd->huf_rc == ZXC_OK && have_huf ? lens : NULL, stream, &dd->g);
+    if (*rc != ZXC_OK) {
+        zxg_dev_free(dd->mem);
+        free(dd);
+        return NULL;
+    }
+    return dd;
+}
+
+uint32_t zxc_b200_dict_device_id(const zxc_b200_dict_device* dd) { return dd ? dd->id : 0; }
+size_t zxc_b200_dict_device_size(const zxc_b200_dict_device* dd) { return dd ? dd->g.dict_size : 0; }
+
+void zxc_b200_dict_device_free(zxc_b200_dict_device* dd) {
+    if (!dd) return;
+    const int prev = zxg_current_device();
+    const int rc = dd->device == prev ? ZXC_OK : zxg_set_device(dd->device);
+    zxg_dev_free(dd->mem); /* waits for the calls that may still read it */
+    if (rc == ZXC_OK && dd->device != prev) zxg_set_device(prev);
+    free(dd);
+}
+
+/* The device check of a device call: a device, and the prepared dictionary's (when given) current */
+static int device_ready(const zxc_b200_dict_device* dd) {
+    const int rc = zxg_init();
+    if (rc != ZXC_OK) return rc;
+    return dd && dd->device != zxg_current_device() ? ZXC_B200_ERROR_NO_DEVICE : ZXC_OK;
+}
+
+/* Each device call has one body for its two entry points: the base call passes its opts, the _using_dict variant opts
+ * without their dictionary fields and the prepared dictionary dd (NULL: none). */
+static const zxc_compress_opts_t* copts_no_dict(const zxc_compress_opts_t* opts, zxc_compress_opts_t* tmp) {
+    if (!opts) return NULL;
+    *tmp = *opts;
+    tmp->dict = NULL;
+    tmp->dict_size = 0;
+    tmp->dict_huf = NULL;
+    return tmp;
+}
+static const zxc_decompress_opts_t* dopts_no_dict(const zxc_decompress_opts_t* opts, zxc_decompress_opts_t* tmp) {
+    if (!opts) return NULL;
+    *tmp = *opts;
+    tmp->dict = NULL;
+    tmp->dict_size = 0;
+    tmp->dict_huf = NULL;
+    return tmp;
+}
+
 /* zxc_compress's option checks, in its order; fills the effective level, block size and block count */
 static int device_opts(uint64_t src_size, const zxc_compress_opts_t* opts, int* level, size_t* block_size,
                        uint32_t* n_blocks) {
@@ -926,6 +1008,34 @@ static int device_opts(uint64_t src_size, const zxc_compress_opts_t* opts, int* 
     return ZXC_OK;
 }
 
+/* The dictionary of a frame compress: opts' host bytes (staged by the call) or the prepared dd */
+typedef struct {
+    const uint8_t* dict;
+    uint32_t dict_size;
+    const zxg_ddict_t* dd;
+    uint32_t id;
+    const uint8_t* huf_lens; /* the host table's unpacked lengths when it is usable (dd carries its own) */
+    uint8_t lens[256];
+} cdict_t;
+/* unpack_dict_huf's verdict on the table, and the rest of *c */
+static int cdict_resolve(const zxc_compress_opts_t* opts, const zxc_b200_dict_device* dd, cdict_t* c) {
+    memset(c, 0, sizeof *c);
+    if (dd) {
+        c->dd = &dd->g;
+        c->id = dd->id;
+        return dd->huf_rc;
+    }
+    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
+    c->dict = opts ? (const uint8_t*)opts->dict : NULL;
+    c->dict_size = (uint32_t)((opts && opts->dict) ? opts->dict_size : 0);
+    int have_huf = 0;
+    const int rc = unpack_dict_huf(dict_huf, c->lens, &have_huf);
+    if (rc != ZXC_OK) return rc;
+    c->huf_lens = have_huf ? c->lens : NULL;
+    c->id = (c->dict && c->dict_size) ? zxc_dict_id(c->dict, c->dict_size, dict_huf) : 0;
+    return ZXC_OK;
+}
+
 size_t zxc_b200_encode_scratch_size(uint64_t src_size, const zxc_compress_opts_t* opts) {
     int level;
     size_t bs;
@@ -935,40 +1045,50 @@ size_t zxc_b200_encode_scratch_size(uint64_t src_size, const zxc_compress_opts_t
     return zxg_encode_scratch_bytes(src_size, (uint32_t)bs, level, nb, (uint32_t)dict_size);
 }
 
-int zxc_b200_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
-                             const zxc_compress_opts_t* opts, void* d_scratch, size_t scratch_size, int64_t* d_result,
-                             zxc_b200_job_t* d_jobs, void* stream) {
+static int compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                           const zxc_compress_opts_t* opts, const zxc_b200_dict_device* dd, void* d_scratch,
+                           size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream) {
     if (!d_dst || dst_capacity == 0 || (src_size > 0 && !d_src) || !d_scratch || !d_result) return ZXC_ERROR_NULL_INPUT;
     int level;
     size_t block_size;
     uint32_t nb;
     int rc = device_opts(src_size, opts, &level, &block_size, &nb);
     if (rc != ZXC_OK) return rc;
-    rc = zxg_init();
+    rc = device_ready(dd);
     if (rc != ZXC_OK) return rc;
     const int checksum = opts ? opts->checksum_enabled : 0;
     const int seekable = opts ? opts->seekable : 0;
-    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
-    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
-    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
     zxg_frame_bytes_t fb;
     memset(&fb, 0, sizeof fb);
     fb.fixed = frame_fixed_bytes(nb, seekable);
     fb.dst_capacity = dst_capacity;
     fb.seekable = seekable && nb > 0;
     if (dst_capacity < fb.fixed) return ZXC_ERROR_DST_TOO_SMALL;
-    uint8_t huf_lens[256];
-    int have_huf = 0;
-    rc = unpack_dict_huf(dict_huf, huf_lens, &have_huf);
+    cdict_t c;
+    rc = cdict_resolve(opts, dd, &c);
     if (rc != ZXC_OK) return rc;
-    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
-    zxf_write_file_header(fb.header, sizeof fb.header, block_size, checksum, did);
+    zxf_write_file_header(fb.header, sizeof fb.header, block_size, checksum, c.id);
     zxf_write_block_header(fb.eof, sizeof fb.eof, ZXF_BT_EOF, 0);
     if (fb.seekable) seek_table_header(fb.sek, nb);
     zxf_write_footer(fb.footer, sizeof fb.footer, src_size, 0, checksum);
-    return zxg_compress_device(d_src, src_size, d_dst, (uint32_t)block_size, level, checksum, nb, dict,
-                               (uint32_t)dict_size, have_huf ? huf_lens : NULL, &fb, d_scratch, scratch_size, d_result,
-                               d_jobs, stream);
+    return zxg_compress_device(d_src, src_size, d_dst, (uint32_t)block_size, level, checksum, nb, c.dict, c.dict_size,
+                               c.huf_lens, c.dd, &fb, d_scratch, scratch_size, d_result, d_jobs, stream);
+}
+
+int zxc_b200_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                             const zxc_compress_opts_t* opts, void* d_scratch, size_t scratch_size, int64_t* d_result,
+                             zxc_b200_job_t* d_jobs, void* stream) {
+    return compress_device(d_src, src_size, d_dst, dst_capacity, opts, NULL, d_scratch, scratch_size, d_result, d_jobs,
+                           stream);
+}
+
+int zxc_b200_compress_device_using_dict(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                                        const zxc_compress_opts_t* opts, const zxc_b200_dict_device* dd,
+                                        void* d_scratch, size_t scratch_size, int64_t* d_result,
+                                        zxc_b200_job_t* d_jobs, void* stream) {
+    zxc_compress_opts_t t;
+    return compress_device(d_src, src_size, d_dst, dst_capacity, copts_no_dict(opts, &t), dd, d_scratch, scratch_size,
+                           d_result, d_jobs, stream);
 }
 
 size_t zxc_b200_compress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_src,
@@ -983,31 +1103,40 @@ size_t zxc_b200_compress_device_batch_scratch_size(uint32_t max_frames, uint64_t
 
 /* The host decides what needs no descriptor, in zxc_b200_compress_device's order; the device makes that call's
  * per-buffer checks and the rest per frame and writes them to d_results (zxc_cbatch.cuh). */
-int zxc_b200_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const zxc_compress_opts_t* opts,
-                                   void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+static int compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const zxc_compress_opts_t* opts,
+                                 const zxc_b200_dict_device* dd, void* d_scratch, size_t scratch_size,
+                                 int64_t* d_results, void* stream) {
     if (n_frames > 0 && (!d_frames || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
     int level;
     size_t block_size;
     uint32_t nb;
     int rc = device_opts(0, opts, &level, &block_size, &nb);
     if (rc != ZXC_OK) return rc;
-    rc = zxg_init();
+    rc = device_ready(dd);
     if (rc != ZXC_OK) return rc;
     const int checksum = opts ? opts->checksum_enabled : 0;
-    const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
-    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
-    const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
-    uint8_t huf_lens[256];
-    int have_huf = 0;
-    rc = unpack_dict_huf(dict_huf, huf_lens, &have_huf);
+    cdict_t c;
+    rc = cdict_resolve(opts, dd, &c);
     if (rc != ZXC_OK || n_frames == 0) return rc;
-    const uint32_t did = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
     uint8_t header[16], eof[8];
-    zxf_write_file_header(header, sizeof header, block_size, checksum, did);
+    zxf_write_file_header(header, sizeof header, block_size, checksum, c.id);
     zxf_write_block_header(eof, sizeof eof, ZXF_BT_EOF, 0);
     return zxg_compress_device_batch(d_frames, n_frames, (uint32_t)block_size, level, checksum,
-                                     opts ? opts->seekable : 0, dict, (uint32_t)dict_size, have_huf ? huf_lens : NULL,
-                                     header, eof, d_scratch, scratch_size, d_results, stream);
+                                     opts ? opts->seekable : 0, c.dict, c.dict_size, c.huf_lens, c.dd, header, eof,
+                                     d_scratch, scratch_size, d_results, stream);
+}
+
+int zxc_b200_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, const zxc_compress_opts_t* opts,
+                                   void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+    return compress_device_batch(d_frames, n_frames, opts, NULL, d_scratch, scratch_size, d_results, stream);
+}
+
+int zxc_b200_compress_device_batch_using_dict(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
+                                              const zxc_compress_opts_t* opts, const zxc_b200_dict_device* dd,
+                                              void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+    zxc_compress_opts_t t;
+    return compress_device_batch(d_frames, n_frames, copts_no_dict(opts, &t), dd, d_scratch, scratch_size, d_results,
+                                 stream);
 }
 
 size_t zxc_b200_decompress_device_scratch_size(uint64_t dst_capacity, uint32_t block_size) {
@@ -1015,8 +1144,19 @@ size_t zxc_b200_decompress_device_scratch_size(uint64_t dst_capacity, uint32_t b
     return zxg_decompress_scratch_bytes(dst_capacity, block_size);
 }
 
-/* The decode options of the device-resident decodes: decompress_frame's dictionary checks that need no frame bytes */
-static int device_dopts(const zxc_decompress_opts_t* opts, zxg_dopts_t* o) {
+/* The decode options of the device-resident decodes: decompress_frame's dictionary checks that need no frame bytes,
+ * for opts' host dictionary or the prepared dd */
+static int device_dopts(const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd, zxg_dopts_t* o) {
+    memset(o, 0, sizeof *o);
+    o->checksum_enabled = opts ? opts->checksum_enabled : 0;
+    if (dd) {
+        o->d_dict = dd->g.dec;
+        o->d_dict_huf = dd->g.dec_huf;
+        o->dict_size = dd->g.dict_size;
+        o->dict_id = dd->id;
+        o->huf_verdict = dd->huf_verdict;
+        return ZXC_OK;
+    }
     const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
     const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
     const uint8_t* dict_huf = (opts && opts->dict) ? (const uint8_t*)opts->dict_huf : NULL;
@@ -1026,23 +1166,36 @@ static int device_dopts(const zxc_decompress_opts_t* opts, zxg_dopts_t* o) {
     o->dict_id = (dict && dict_size) ? zxc_dict_id(dict, dict_size, dict_huf) : 0;
     o->huf_verdict = dict_size ? dict_huf_attach(dict_huf) : 0;
     o->dict_huf = o->huf_verdict == 1 ? dict_huf : NULL;
-    o->checksum_enabled = opts ? opts->checksum_enabled : 0;
     return ZXC_OK;
 }
 
 /* The host decides what needs no frame bytes, in zxc_decompress's order (decompress_entry, decompress_frame); the
  * device decides the rest and writes it to *d_result (zxc_dplan.cuh). */
-int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
-                               const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
-                               int64_t* d_result, void* stream) {
+static int decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                             const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd, void* d_scratch,
+                             size_t scratch_size, int64_t* d_result, void* stream) {
     if (!d_src || (!d_dst && dst_capacity != 0) || !d_scratch || !d_result) return ZXC_ERROR_NULL_INPUT;
     if (src_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE) return ZXC_ERROR_SRC_TOO_SMALL;
     zxg_dopts_t o;
-    const int orc = device_dopts(opts, &o);
+    const int orc = device_dopts(opts, dd, &o);
     if (orc != ZXC_OK) return orc;
-    const int irc = zxg_init();
+    const int irc = device_ready(dd);
     if (irc != ZXC_OK) return irc;
     return zxg_decompress_device(d_src, src_size, d_dst, dst_capacity, &o, d_scratch, scratch_size, d_result, stream);
+}
+
+int zxc_b200_decompress_device(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                               const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                               int64_t* d_result, void* stream) {
+    return decompress_device(d_src, src_size, d_dst, dst_capacity, opts, NULL, d_scratch, scratch_size, d_result, stream);
+}
+
+int zxc_b200_decompress_device_using_dict(const void* d_src, uint64_t src_size, void* d_dst, uint64_t dst_capacity,
+                                          const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd,
+                                          void* d_scratch, size_t scratch_size, int64_t* d_result, void* stream) {
+    zxc_decompress_opts_t t;
+    return decompress_device(d_src, src_size, d_dst, dst_capacity, dopts_no_dict(opts, &t), dd, d_scratch,
+                             scratch_size, d_result, stream);
 }
 
 size_t zxc_b200_decompress_inplace_device_scratch_size(uint64_t buffer_capacity, uint32_t block_size, uint64_t window) {
@@ -1061,19 +1214,35 @@ size_t zxc_b200_decompress_inplace_device_bound(const void* d_src, uint64_t src_
 
 /* The host decides what zxc_decompress_inplace decides without the frame's bytes, then what
  * zxc_b200_decompress_device decides without them; the device decides the rest (zxc_dinplace.cuh). */
-int zxc_b200_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,
-                                       const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
-                                       int64_t* d_result, void* stream) {
+static int decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,
+                                     const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd,
+                                     void* d_scratch, size_t scratch_size, int64_t* d_result, void* stream) {
     if (!d_buffer || comp_size < ZXC_FILE_HEADER_SIZE + ZXC_FILE_FOOTER_SIZE || comp_size > buffer_capacity ||
         !d_scratch || !d_result)
         return ZXC_ERROR_NULL_INPUT;
     zxg_dopts_t o;
-    const int orc = device_dopts(opts, &o);
+    const int orc = device_dopts(opts, dd, &o);
     if (orc != ZXC_OK) return orc;
-    const int irc = zxg_init();
+    const int irc = device_ready(dd);
     if (irc != ZXC_OK) return irc;
     return zxg_decompress_inplace_device(d_buffer, buffer_capacity, comp_size, &o, d_scratch, scratch_size, d_result,
                                          stream);
+}
+
+int zxc_b200_decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,
+                                       const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
+                                       int64_t* d_result, void* stream) {
+    return decompress_inplace_device(d_buffer, buffer_capacity, comp_size, opts, NULL, d_scratch, scratch_size,
+                                     d_result, stream);
+}
+
+int zxc_b200_decompress_inplace_device_using_dict(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,
+                                                  const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd,
+                                                  void* d_scratch, size_t scratch_size, int64_t* d_result,
+                                                  void* stream) {
+    zxc_decompress_opts_t t;
+    return decompress_inplace_device(d_buffer, buffer_capacity, comp_size, dopts_no_dict(opts, &t), dd, d_scratch,
+                                     scratch_size, d_result, stream);
 }
 
 size_t zxc_b200_decompress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_capacity,
@@ -1084,16 +1253,31 @@ size_t zxc_b200_decompress_device_batch_scratch_size(uint32_t max_frames, uint64
 
 /* The host decides what needs neither the descriptors nor the frames' bytes; the device decides the rest per frame
  * and writes it to d_results (zxc_dbatch.cuh). */
+static int decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
+                                   const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd, void* d_scratch,
+                                   size_t scratch_size, int64_t* d_results, void* stream) {
+    if (n_frames > 0 && (!d_frames || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
+    zxg_dopts_t o;
+    const int orc = device_dopts(opts, dd, &o);
+    if (orc != ZXC_OK) return orc;
+    const int irc = device_ready(dd);
+    if (irc != ZXC_OK || n_frames == 0) return irc;
+    return zxg_decompress_device_batch(d_frames, n_frames, &o, d_scratch, scratch_size, d_results, stream);
+}
+
 int zxc_b200_decompress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
                                      const zxc_decompress_opts_t* opts, void* d_scratch, size_t scratch_size,
                                      int64_t* d_results, void* stream) {
-    if (n_frames > 0 && (!d_frames || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
-    zxg_dopts_t o;
-    const int orc = device_dopts(opts, &o);
-    if (orc != ZXC_OK) return orc;
-    const int irc = zxg_init();
-    if (irc != ZXC_OK || n_frames == 0) return irc;
-    return zxg_decompress_device_batch(d_frames, n_frames, &o, d_scratch, scratch_size, d_results, stream);
+    return decompress_device_batch(d_frames, n_frames, opts, NULL, d_scratch, scratch_size, d_results, stream);
+}
+
+int zxc_b200_decompress_device_batch_using_dict(const zxc_b200_frame_t* d_frames, uint32_t n_frames,
+                                                const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd,
+                                                void* d_scratch, size_t scratch_size, int64_t* d_results,
+                                                void* stream) {
+    zxc_decompress_opts_t t;
+    return decompress_device_batch(d_frames, n_frames, dopts_no_dict(opts, &t), dd, d_scratch, scratch_size,
+                                   d_results, stream);
 }
 
 /* ---- the block API in HBM: zxc_compress_block / zxc_decompress_block(_safe) over a batch ---- */
@@ -1107,34 +1291,64 @@ size_t zxc_b200_compress_blocks_device_scratch_size(uint32_t max_blocks, uint64_
 
 /* The host decides what needs no descriptor; the device makes zxc_compress_block's per-item checks and the rest and
  * writes them to d_results (zxc_blocks.cuh).  The options resolve as on a fresh zxc_create_cctx(NULL) context. */
-int zxc_b200_compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, const zxc_compress_opts_t* opts,
-                                    void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+static int compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, const zxc_compress_opts_t* opts,
+                                  const zxc_b200_dict_device* dd, void* d_scratch, size_t scratch_size,
+                                  int64_t* d_results, void* stream) {
     if (n_items > 0 && (!d_items || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
     const uint8_t* dict = opts ? (const uint8_t*)opts->dict : NULL;
     const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
     if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
-    const int irc = zxg_init();
+    const int irc = device_ready(dd);
     if (irc != ZXC_OK || n_items == 0) return irc;
     return zxg_compress_blocks_device(d_items, n_items, level_clamp(opts ? opts->level : 0),
-                                      opts ? opts->checksum_enabled : 0, dict, (uint32_t)dict_size, d_scratch,
-                                      scratch_size, d_results, stream);
+                                      opts ? opts->checksum_enabled : 0, dict, (uint32_t)dict_size,
+                                      dd ? &dd->g : NULL, d_scratch, scratch_size, d_results, stream);
+}
+
+int zxc_b200_compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, const zxc_compress_opts_t* opts,
+                                    void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+    return compress_blocks_device(d_items, n_items, opts, NULL, d_scratch, scratch_size, d_results, stream);
+}
+
+int zxc_b200_compress_blocks_device_using_dict(const zxc_b200_frame_t* d_items, uint32_t n_items,
+                                               const zxc_compress_opts_t* opts, const zxc_b200_dict_device* dd,
+                                               void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+    zxc_compress_opts_t t;
+    return compress_blocks_device(d_items, n_items, copts_no_dict(opts, &t), dd, d_scratch, scratch_size, d_results,
+                                  stream);
 }
 
 size_t zxc_b200_decompress_blocks_device_scratch_size(uint32_t max_blocks, uint64_t max_dst_capacity) {
     return zxg_decompress_blocks_scratch_bytes(max_blocks, max_dst_capacity);
 }
 
+static int decompress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items,
+                                    const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd, int safe,
+                                    void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
+    if (n_items > 0 && (!d_items || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
+    zxg_dopts_t o;
+    const int orc = device_dopts(opts, dd, &o);
+    if (orc != ZXC_OK) return orc;
+    o.dict_huf = NULL; /* the block API attaches no literal table (decode_one_block) */
+    o.d_dict_huf = NULL;
+    const int irc = device_ready(dd);
+    if (irc != ZXC_OK || n_items == 0) return irc;
+    return zxg_decompress_blocks_device(d_items, n_items, &o, safe, d_scratch, scratch_size, d_results, stream);
+}
+
 int zxc_b200_decompress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items,
                                       const zxc_decompress_opts_t* opts, int safe, void* d_scratch,
                                       size_t scratch_size, int64_t* d_results, void* stream) {
-    if (n_items > 0 && (!d_items || !d_results || !d_scratch)) return ZXC_ERROR_NULL_INPUT;
-    zxg_dopts_t o;
-    const int orc = device_dopts(opts, &o);
-    if (orc != ZXC_OK) return orc;
-    o.dict_huf = NULL; /* the block API attaches no literal table (decode_one_block) */
-    const int irc = zxg_init();
-    if (irc != ZXC_OK || n_items == 0) return irc;
-    return zxg_decompress_blocks_device(d_items, n_items, &o, safe, d_scratch, scratch_size, d_results, stream);
+    return decompress_blocks_device(d_items, n_items, opts, NULL, safe, d_scratch, scratch_size, d_results, stream);
+}
+
+int zxc_b200_decompress_blocks_device_using_dict(const zxc_b200_frame_t* d_items, uint32_t n_items,
+                                                 const zxc_decompress_opts_t* opts, const zxc_b200_dict_device* dd,
+                                                 int safe, void* d_scratch, size_t scratch_size, int64_t* d_results,
+                                                 void* stream) {
+    zxc_decompress_opts_t t;
+    return decompress_blocks_device(d_items, n_items, dopts_no_dict(opts, &t), dd, safe, d_scratch, scratch_size,
+                                    d_results, stream);
 }
 
 int64_t zxc_compress_cctx(zxc_cctx* cctx, const void* src, size_t src_size, void* dst, size_t dst_capacity,

@@ -1064,10 +1064,13 @@ extern "C" int zxg_decode_staged(zxg_ctx* c, const uint8_t* h_src, zxg_fetch_fn 
 /* ------------------------------------------------------------------------- */
 static u32 enc_staging_stride(u32 bs) { return ((bs + 8u + 68u + 4u) + 255u) & ~255u; }
 
-/* dictionary region of an encode: [dict (padded)] [seeded head 128 KB] [seeded chain 128 KB] [256 literal lengths] */
+/* dictionary region of an encode: [dict (padded)] [seeded head 128 KB] [seeded chain 128 KB] [256 literal lengths];
+ * a prepared dictionary's region holds two head / chain pairs (zxc_seed_kernel depends on the level only through
+ * hash5 = level >= 3): enc_dict_bytes(dict_size, 2) */
+static const size_t ENC_SEED_PAIR = (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2;
 static size_t enc_dict_pad(u32 dict_size) { return ((size_t)dict_size + 16 + 255) & ~(size_t)255; }
-static size_t enc_dict_bytes(u32 dict_size) {
-    return enc_dict_pad(dict_size) + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2 + 256;
+static size_t enc_dict_bytes(u32 dict_size, u32 pairs = 1) {
+    return enc_dict_pad(dict_size) + pairs * ENC_SEED_PAIR + 256;
 }
 
 /* warps of the full resident encode grid for n_blocks blocks (a multiple of ENC_WARPS_PER_CTA) */
@@ -1080,7 +1083,8 @@ static u32 enc_full_warps(u32 n_blocks) {
 /* One block encode on stream `st` with the given device buffers: d_src is 16-byte aligned with 64 zero bytes behind
  * src_size, d_scratch holds `warps` per-warp slots of enc_layout(block_size, level).total bytes, d_dict (when
  * dict_size) holds enc_dict_bytes(dict_size).  The host dictionary (<= ZXC_DICT_SIZE_MAX bytes) and literal lengths
- * are copied in here.  Launches the seed kernel (dictionary only) and the encode kernel: `warps` warps, in CTAs of
+ * are copied in here, unless a prepared dictionary dd is given.  Launches the seed kernel (host dictionary only) and
+ * the encode kernel: `warps` warps, in CTAs of
  * ENC_WARPS_PER_CTA when there are that many, else one CTA of `warps` warps (the kernel indexes its scratch by
  * global warp and claims blocks through *counter, so any warp count gives the same output). */
 struct EncLaunch {
@@ -1097,32 +1101,58 @@ struct EncLaunch {
     const void* h_dict;
     u32 dict_size;
     const uint8_t* h_dict_huf_lens;
+    const zxg_ddict_t* dd; /* or a prepared dictionary (h_dict NULL) */
 };
-/* The dictionary region of an encode at d_dict (enc_dict_bytes(dict_size) bytes): the host dictionary, read through a
- * pageable copy (host_bounce) so the call has read it when it returns, and at level 6-7 the literal lengths, copied in;
- * the match tables seeded by zxc_seed_kernel (one launch).  Fills P's dictionary fields. */
+/* Builds the dictionary region of an encode at d_dict (enc_dict_bytes(dict_size, pairs) bytes): the host dictionary,
+ * read through a pageable copy (host_bounce) so the call has read it when it returns, and the literal lengths when
+ * given, copied in; head / chain pair k seeded by zxc_seed_kernel for levels[k] (one launch each). */
 static void* host_bounce(const void* p, size_t n, size_t bytes);
-static int enc_stage_dict(EncodeParams& P, u8* d_dict, const void* h_dict, u32 dict_size, int level,
+static int enc_build_dict(u8* d_dict, const void* h_dict, u32 dict_size, const int* levels, u32 pairs,
                           const uint8_t* h_dict_huf_lens, cudaStream_t st) {
     void* bd = host_bounce(h_dict, dict_size, dict_size);
     if (!bd) return ZXC_ERROR_MEMORY;
     const size_t dpad = enc_dict_pad(dict_size);
-    const bool ok = cudaMemsetAsync(d_dict, 0, enc_dict_bytes(dict_size), st) == cudaSuccess &&
+    const bool ok = cudaMemsetAsync(d_dict, 0, enc_dict_bytes(dict_size, pairs), st) == cudaSuccess &&
                     cudaMemcpyAsync(d_dict, bd, dict_size, cudaMemcpyHostToDevice, st) == cudaSuccess;
     free(bd);
     if (!ok) return ZXC_B200_ERROR_CUDA;
-    P.dict = d_dict;
-    P.seed_head = (const u32*)(d_dict + dpad);
-    P.seed_chain = (const unsigned short*)(d_dict + dpad + (size_t)ENC_HASH_SIZE * 4);
-    if (h_dict_huf_lens && level >= 6) { /* the shared literal table, one length per byte */
-        u8* d_lens = d_dict + dpad + (size_t)ENC_HASH_SIZE * 4 + (size_t)ENC_WINDOW * 2;
-        if (cudaMemcpyAsync(d_lens, h_dict_huf_lens, 256, cudaMemcpyHostToDevice, st) != cudaSuccess)
-            return ZXC_B200_ERROR_CUDA;
-        P.dict_huf_lens = d_lens;
+    if (h_dict_huf_lens && /* the shared literal table, one length per byte */
+        cudaMemcpyAsync(d_dict + dpad + pairs * ENC_SEED_PAIR, h_dict_huf_lens, 256, cudaMemcpyHostToDevice, st) !=
+            cudaSuccess)
+        return ZXC_B200_ERROR_CUDA;
+    for (u32 k = 0; k < pairs; k++) {
+        u8* pair = d_dict + dpad + k * ENC_SEED_PAIR;
+        zxc_seed_kernel<<<1, 32, 0, st>>>(d_dict, dict_size, (u32)levels[k], (u32*)pair,
+                                          (unsigned short*)(pair + (size_t)ENC_HASH_SIZE * 4));
+        __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     }
-    zxc_seed_kernel<<<1, 32, 0, st>>>(d_dict, dict_size, (u32)level, (u32*)P.seed_head, (unsigned short*)P.seed_chain);
-    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return ZXC_OK;
+}
+
+/* Points P's dictionary fields at a region laid out by enc_build_dict: head / chain pair `pair`, the literal lengths
+ * when has_lens and the level reads them (6-7). */
+static void enc_point_dict(EncodeParams& P, const u8* d_dict, u32 dict_size, u32 pairs, u32 pair, bool has_lens,
+                           int level) {
+    const u8* seeds = d_dict + enc_dict_pad(dict_size);
+    P.dict = d_dict;
+    P.seed_head = (const u32*)(seeds + pair * ENC_SEED_PAIR);
+    P.seed_chain = (const unsigned short*)(seeds + pair * ENC_SEED_PAIR + (size_t)ENC_HASH_SIZE * 4);
+    if (has_lens && level >= 6) P.dict_huf_lens = seeds + pairs * ENC_SEED_PAIR;
+}
+
+/* The dictionary of an encode at this level, into P: the host dictionary staged into the region at d_dict (one
+ * seeding launch), or the prepared dictionary dd used where it lies (no launch); with_lens: dd's literal lengths apply
+ * (the block API attaches none). */
+static int enc_stage_dict(EncodeParams& P, u8* d_dict, const void* h_dict, u32 dict_size, int level,
+                          const uint8_t* h_dict_huf_lens, const zxg_ddict_t* dd, bool with_lens, cudaStream_t st) {
+    if (dd) {
+        enc_point_dict(P, (const u8*)dd->enc, dd->dict_size, 2, level >= 3 ? 1 : 0, with_lens && dd->enc_lens, level);
+        return ZXC_OK;
+    }
+    const uint8_t* lens = level >= 6 ? h_dict_huf_lens : NULL;
+    const int rc = enc_build_dict(d_dict, h_dict, dict_size, &level, 1, lens, st);
+    if (rc == ZXC_OK) enc_point_dict(P, d_dict, dict_size, 1, 0, lens != NULL, level);
+    return rc;
 }
 
 static int launch_encode(const EncLaunch& E, cudaStream_t st) {
@@ -1136,8 +1166,8 @@ static int launch_encode(const EncLaunch& E, cudaStream_t st) {
     P.seed_head = NULL;
     P.seed_chain = NULL;
     P.dict_huf_lens = NULL;
-    if (E.h_dict && E.dict_size) {
-        const int rc = enc_stage_dict(P, E.d_dict, E.h_dict, E.dict_size, E.level, E.h_dict_huf_lens, st);
+    if (E.dd || (E.h_dict && E.dict_size)) {
+        const int rc = enc_stage_dict(P, E.d_dict, E.h_dict, E.dict_size, E.level, E.h_dict_huf_lens, E.dd, true, st);
         if (rc != ZXC_OK) return rc;
     }
     P.src_size = E.src_size;
@@ -1147,7 +1177,7 @@ static int launch_encode(const EncLaunch& E, cudaStream_t st) {
     P.staging_stride = enc_staging_stride(E.block_size);
     P.level = (u32)E.level;
     P.checksum = E.checksum ? 1u : 0u;
-    P.dict_size = P.dict ? E.dict_size : 0;
+    P.dict_size = P.dict ? (E.dd ? E.dd->dict_size : E.dict_size) : 0;
     if (cudaMemsetAsync(E.counter, 0, sizeof(unsigned long long), st) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
     const u32 grid = E.warps >= ENC_WARPS_PER_CTA ? E.warps / ENC_WARPS_PER_CTA : 1u;
     const u32 threads = E.warps >= ENC_WARPS_PER_CTA ? ENC_CTA_THREADS : 32u * E.warps;
@@ -1193,7 +1223,7 @@ extern "C" int zxg_encode_body(zxg_ctx* c, const uint8_t* h_src, uint64_t src_si
         if (!d_dict) return ZXC_ERROR_MEMORY;
     }
     const EncLaunch E = {d_src, src_size, block_size, n_blocks, level, checksum, d_stage, d_sizes, d_scratch, warps,
-                         c->counter, d_dict, h_dict, dict_size, h_dict_huf_lens};
+                         c->counter, d_dict, h_dict, dict_size, h_dict_huf_lens, NULL};
     rc = launch_encode(E, c->stream);
     if (rc != ZXC_OK) return rc;
     if (cudaMemcpyAsync(h_sizes, d_sizes, (size_t)n_blocks * 4, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
@@ -1279,8 +1309,9 @@ extern "C" size_t zxg_encode_scratch_bytes(uint64_t src_size, uint32_t block_siz
 
 extern "C" int zxg_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint32_t block_size, int level,
                                    int checksum, uint32_t n_blocks, const void* h_dict, uint32_t dict_size,
-                                   const uint8_t* h_dict_huf_lens, const zxg_frame_bytes_t* fb, void* d_scratch,
-                                   size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream) {
+                                   const uint8_t* h_dict_huf_lens, const zxg_ddict_t* dd, const zxg_frame_bytes_t* fb,
+                                   void* d_scratch, size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs,
+                                   void* stream) {
     const int irc = zxg_init();
     if (irc != ZXC_OK) return irc;
     const DevEncLayout L = dev_enc_layout(src_size, block_size, n_blocks, level, dict_size);
@@ -1316,7 +1347,7 @@ extern "C" int zxg_compress_device(const void* d_src, uint64_t src_size, void* d
             cudaMemsetAsync(d_in + src_size, 0, 64, st) != cudaSuccess)
             return ZXC_B200_ERROR_CUDA;
         const EncLaunch E = {d_in, src_size, block_size, n_blocks, level, checksum, d_stage, d_sizes, base + L.warps,
-                             warps, &state->counter, base + L.dict, h_dict, dict_size, h_dict_huf_lens};
+                             warps, &state->counter, base + L.dict, h_dict, dict_size, h_dict_huf_lens, dd};
         const int rc = launch_encode(E, st);
         if (rc != ZXC_OK) return rc;
         zxc_asm_tile_sums<<<n_tiles, ASM_THREADS, 0, st>>>(d_sizes, n_blocks, d_tiles);
@@ -1401,9 +1432,9 @@ extern "C" size_t zxg_compress_batch_scratch_bytes(uint32_t max_frames, uint64_t
 
 extern "C" int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, uint32_t block_size,
                                          int level, int checksum, int seekable, const void* h_dict,
-                                         uint32_t dict_size, const uint8_t* h_dict_huf_lens, const uint8_t* header,
-                                         const uint8_t* eof, void* d_scratch, size_t scratch_size, int64_t* d_results,
-                                         void* stream) {
+                                         uint32_t dict_size, const uint8_t* h_dict_huf_lens, const zxg_ddict_t* dd,
+                                         const uint8_t* header, const uint8_t* eof, void* d_scratch,
+                                         size_t scratch_size, int64_t* d_results, void* stream) {
     const int irc = zxg_init();
     if (irc != ZXC_OK) return irc;
     const u32 n = n_frames;
@@ -1451,8 +1482,8 @@ extern "C" int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint3
     /* the W encode slots end at the room's end: slot g at scratch + g * wstride; those below the room never run */
     P.scratch = A.staging + (size_t)L.pool_units * 256 + L.wstride - (size_t)L.W * L.wstride;
     P.counter = &A.st->counter;
-    if (dsz) {
-        const int rc = enc_stage_dict(P, base + L.dict, h_dict, dsz, level, h_dict_huf_lens, st);
+    if (dd || dsz) {
+        const int rc = enc_stage_dict(P, base + L.dict, h_dict, dsz, level, h_dict_huf_lens, dd, true, st);
         if (rc != ZXC_OK) return rc;
     }
     P.scratch_stride = L.wstride;
@@ -1460,7 +1491,7 @@ extern "C" int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint3
     P.staging_stride = L.stride;
     P.level = (u32)level;
     P.checksum = A.checksum;
-    P.dict_size = dsz;
+    P.dict_size = dd ? dd->dict_size : dsz;
     const u32 sms = (u32)(g_sm_count > 0 ? g_sm_count : 132);
     const u32 n_tiles = (n + ASM_TILE - 1) / ASM_TILE;
     const u32 per_frame = (n + CB_THREADS - 1) / CB_THREADS;
@@ -1497,25 +1528,30 @@ extern "C" int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint3
  * J = ceil(dst_capacity / ZXC_BLOCK_SIZE_MIN) + 2: every block but the last of a frame the reference's encoder
  * writes holds block_size >= ZXC_BLOCK_SIZE_MIN bytes, so such a frame fits the table when its output fits
  * dst_capacity. */
-/* A decode's dictionary and its literal table (when given) into the scratch's dictionary region at d_region, through
- * a pageable host copy: the caller's dictionary has been read when the call returns, whatever memory it is in
- * (host_bounce).  Both device pointers stay NULL without a dictionary. */
-static int dec_stage_dict(u8* d_region, const zxg_dopts_t* o, cudaStream_t st, u8** d_dict, u8** d_huf) {
-    *d_dict = NULL;
-    *d_huf = NULL;
-    const u32 dict_size = o->dict_size;
-    if (!o->dict || !dict_size) return ZXC_OK;
-    *d_dict = d_region;
-    const size_t dbytes = (size_t)dict_size + (o->dict_huf ? ZXC_HUF_TABLE_SIZE : 0);
-    u8* b = (u8*)host_bounce(o->dict, dict_size, dbytes);
+/* Builds a decode's dictionary region at d_region: the dictionary, then its literal table when h_huf is given, through
+ * a pageable host copy, so the caller's dictionary has been read when the call returns, whatever memory it is in
+ * (host_bounce). */
+static int dec_build_dict(u8* d_region, const void* h_dict, u32 dict_size, const void* h_huf, cudaStream_t st) {
+    const size_t dbytes = (size_t)dict_size + (h_huf ? ZXC_HUF_TABLE_SIZE : 0);
+    u8* b = (u8*)host_bounce(h_dict, dict_size, dbytes);
     if (!b) return ZXC_ERROR_MEMORY;
-    if (o->dict_huf) {
-        memcpy(b + dict_size, o->dict_huf, ZXC_HUF_TABLE_SIZE);
-        *d_huf = d_region + dict_size;
-    }
+    if (h_huf) memcpy(b + dict_size, h_huf, ZXC_HUF_TABLE_SIZE);
     const cudaError_t e = cudaMemcpyAsync(d_region, b, dbytes, cudaMemcpyHostToDevice, st);
     free(b);
     return e == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* A decode's dictionary and its literal table (when given): a prepared dictionary's decode region where it lies, or
+ * the host dictionary built into the scratch's dictionary region at d_region.  Both device pointers stay NULL without
+ * a dictionary. */
+static int dec_stage_dict(u8* d_region, const zxg_dopts_t* o, cudaStream_t st, u8** d_dict, u8** d_huf) {
+    *d_dict = (u8*)o->d_dict;
+    *d_huf = (u8*)o->d_dict_huf;
+    const u32 dict_size = o->dict_size;
+    if (!o->dict || !dict_size) return ZXC_OK;
+    *d_dict = d_region;
+    if (o->dict_huf) *d_huf = d_region + dict_size;
+    return dec_build_dict(d_region, o->dict, dict_size, o->dict_huf, st);
 }
 
 /* the device's share of the decode options, for a scratch sized for block size bs */
@@ -1523,7 +1559,7 @@ static DDecodeOpts dec_opts(const zxg_dopts_t* o, u32 bs) {
     DDecodeOpts d;
     d.max_block_size = bs;
     d.dict_id = o->dict_id;
-    d.have_dict = o->dict && o->dict_size ? 1u : 0u;
+    d.have_dict = (o->dict || o->d_dict) && o->dict_size ? 1u : 0u;
     d.huf_verdict = o->huf_verdict;
     d.checksum_enabled = o->checksum_enabled ? 1u : 0u;
     return d;
@@ -2024,8 +2060,8 @@ extern "C" size_t zxg_compress_blocks_scratch_bytes(uint32_t max_blocks, uint64_
 }
 
 extern "C" int zxg_compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, int level, int checksum,
-                                          const void* h_dict, uint32_t dict_size, void* d_scratch, size_t scratch_size,
-                                          int64_t* d_results, void* stream) {
+                                          const void* h_dict, uint32_t dict_size, const zxg_ddict_t* dd,
+                                          void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream) {
     const int irc = zxg_init();
     if (irc != ZXC_OK) return irc;
     const u32 n = n_items;
@@ -2050,13 +2086,13 @@ extern "C" int zxg_compress_blocks_device(const zxc_b200_frame_t* d_items, uint3
     EncodeParams P;
     memset(&P, 0, sizeof P);
     P.counter = &A.st->counter;
-    if (dsz) { /* the block API attaches no shared literal table */
-        const int rc = enc_stage_dict(P, base + dict, h_dict, dsz, level, NULL, st);
+    if (dd || dsz) { /* the block API attaches no shared literal table */
+        const int rc = enc_stage_dict(P, base + dict, h_dict, dsz, level, NULL, dd, false, st);
         if (rc != ZXC_OK) return rc;
     }
     P.level = (u32)level;
     P.checksum = checksum ? 1u : 0u;
-    P.dict_size = dsz;
+    P.dict_size = dd ? dd->dict_size : dsz;
     const u32 sms = (u32)(g_sm_count > 0 ? g_sm_count : 132);
     const u32 n_tiles = (n + ASM_TILE - 1) / ASM_TILE;
     const u32 by_warp = (n + BK_THREADS / 32 - 1) / (BK_THREADS / 32);
@@ -2309,6 +2345,32 @@ extern "C" void zxg_dev_free(void* d) {
     if (!d) return;
     cudaDeviceSynchronize(); /* range calls still in flight on any stream may read it */
     cudaFree(d);
+}
+
+/* ---- prepared dictionaries (zxc_b200_dict_device: zxc_api.c): the decode region, then the encode region ---- */
+static size_t ddict_enc_off(u32 dict_size) { return r256((size_t)dict_size + ZXC_HUF_TABLE_SIZE); }
+
+extern "C" size_t zxg_ddict_bytes(uint32_t dict_size) { return ddict_enc_off(dict_size) + enc_dict_bytes(dict_size, 2); }
+
+extern "C" int zxg_ddict_build(void* d_base, const void* h_dict, uint32_t dict_size, const void* h_dec_huf,
+                               const uint8_t* h_lens, void* stream, zxg_ddict_t* dd) {
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)d_base;
+    u8* enc = base + ddict_enc_off(dict_size);
+    static const int seed_levels[2] = {1, 3}; /* hash5 off, on */
+    int rc = dec_build_dict(base, h_dict, dict_size, h_dec_huf, st);
+    if (rc == ZXC_OK) rc = enc_build_dict(enc, h_dict, dict_size, seed_levels, 2, h_lens, st);
+    if (rc == ZXC_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = ZXC_B200_ERROR_CUDA;
+    if (rc != ZXC_OK) {
+        cudaGetLastError();
+        return rc;
+    }
+    dd->dec = base;
+    dd->dec_huf = h_dec_huf ? base + dict_size : NULL;
+    dd->enc = enc;
+    dd->enc_lens = h_lens ? enc + enc_dict_pad(dict_size) + 2 * ENC_SEED_PAIR : NULL;
+    dd->dict_size = dict_size;
+    return ZXC_OK;
 }
 
 /* Scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned):

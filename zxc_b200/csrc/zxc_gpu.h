@@ -51,8 +51,28 @@ int zxg_encode_body(zxg_ctx* c, const uint8_t* h_src, uint64_t src_size, uint32_
                     int checksum, uint32_t n_blocks, uint8_t* h_body, uint64_t body_cap, uint32_t* h_sizes,
                     uint64_t* body_size, const void* h_dict, uint32_t dict_size, const uint8_t* h_dict_huf_lens);
 
+/* A prepared dictionary in device memory (zxc_b200_dict_device): one allocation of zxg_ddict_bytes(dict_size) bytes
+ * with the regions the per-call staging builds, made once by zxg_ddict_build and only read after that.
+ *   decode region: the content, then its 128-byte table when one was given (dec_huf != NULL): dec_stage_dict's region
+ *   encode region: the content zero-padded, one seeded head / chain pair per hash (levels 1-2, levels 3-7), then the
+ *                  256 literal lengths when enc_lens != NULL: enc_stage_dict's region, with two pairs */
+typedef struct {
+    const void* dec;
+    const void* dec_huf;
+    const void* enc;
+    const void* enc_lens;
+    uint32_t dict_size;
+} zxg_ddict_t;
+size_t zxg_ddict_bytes(uint32_t dict_size);
+/* Builds both regions at d_base from host bytes (h_dec_huf: the table the decode region carries, or NULL; h_lens: the
+ * 256 unpacked lengths, or NULL) on `stream` and waits for them; fills *dd. */
+int zxg_ddict_build(void* d_base, const void* h_dict, uint32_t dict_size, const void* h_dec_huf, const uint8_t* h_lens,
+                    void* stream, zxg_ddict_t* dd);
+
 /* Device-to-device compress (zxc_b200_compress_device).  The host writes the frame's fixed bytes with the
- * zxc_format.c helpers; the device places them around the body it assembles. */
+ * zxc_format.c helpers; the device places them around the body it assembles.  The compress calls below take their
+ * dictionary as host bytes (h_dict, staged per call into the scratch's dictionary region) or as a prepared dictionary
+ * dd (then h_dict is NULL, dict_size 0, and the layout has no dictionary region). */
 typedef struct {
     uint8_t header[16];    /* file header */
     uint8_t eof[8];        /* EOF block header */
@@ -68,14 +88,16 @@ size_t zxg_encode_scratch_bytes(uint64_t src_size, uint32_t block_size, int leve
 /* enqueues the copy, encode and assembly on `stream`; ZXC_ERROR_MEMORY when the scratch holds less than one warp */
 int zxg_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint32_t block_size, int level,
                         int checksum, uint32_t n_blocks, const void* h_dict, uint32_t dict_size,
-                        const uint8_t* h_dict_huf_lens, const zxg_frame_bytes_t* fb, void* d_scratch,
-                        size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
+                        const uint8_t* h_dict_huf_lens, const zxg_ddict_t* dd, const zxg_frame_bytes_t* fb,
+                        void* d_scratch, size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
 
 /* The decode options of a device-resident decode, resolved on the host from zxc_decompress_opts_t: what needs no
  * frame bytes. */
 typedef struct {
     const void* dict;     /* NULL without a dictionary; copied into the scratch */
     const void* dict_huf; /* its literal table, NULL unless dict_huf_attach finds it usable */
+    const void* d_dict;   /* or a prepared dictionary's decode region (dict is then NULL): used where it lies */
+    const void* d_dict_huf;
     uint32_t dict_size;
     uint32_t dict_id;     /* zxc_dict_id of the dictionary */
     int huf_verdict;      /* dict_huf_attach of its table: 1 usable, 0 none, < 0 malformed */
@@ -114,8 +136,9 @@ size_t zxg_compress_batch_scratch_bytes(uint32_t max_frames, uint64_t max_total_
                                         uint32_t dict_size);
 int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frames, uint32_t block_size, int level,
                               int checksum, int seekable, const void* h_dict, uint32_t dict_size,
-                              const uint8_t* h_dict_huf_lens, const uint8_t* header, const uint8_t* eof,
-                              void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);
+                              const uint8_t* h_dict_huf_lens, const zxg_ddict_t* dd, const uint8_t* header,
+                              const uint8_t* eof, void* d_scratch, size_t scratch_size, int64_t* d_results,
+                              void* stream);
 
 /* The block API in HBM (zxc_b200_compress_blocks_device, zxc_b200_decompress_blocks_device; kernels in
  * zxc_blocks.cuh), with the options checked by the host.  Scratch sizes (0 without a device or when that cannot be
@@ -123,8 +146,8 @@ int zxg_compress_device_batch(const zxc_b200_frame_t* d_frames, uint32_t n_frame
 size_t zxg_compress_blocks_scratch_bytes(uint32_t max_blocks, uint64_t max_total_src, uint32_t max_src_size, int level,
                                          uint32_t dict_size);
 int zxg_compress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, int level, int checksum,
-                               const void* h_dict, uint32_t dict_size, void* d_scratch, size_t scratch_size,
-                               int64_t* d_results, void* stream);
+                               const void* h_dict, uint32_t dict_size, const zxg_ddict_t* dd, void* d_scratch,
+                               size_t scratch_size, int64_t* d_results, void* stream);
 size_t zxg_decompress_blocks_scratch_bytes(uint32_t max_blocks, uint64_t max_dst_capacity);
 int zxg_decompress_blocks_device(const zxc_b200_frame_t* d_items, uint32_t n_items, const zxg_dopts_t* o, int safe,
                                  void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);

@@ -9,8 +9,10 @@ in one zxc_b200_decompress_device_batch call, and ``compress_frames`` compresses
 one zxc_b200_compress_device_batch call.  ``decompress_inplace`` decodes a frame that lies flush-right in a CUDA buffer
 into the same buffer with zxc_b200_decompress_inplace_device, and ``load_frame`` uses it to bring a frame from the
 host into HBM and expand it there with no second buffer.  ``compress_blocks`` and ``decompress_blocks`` are the block
-API in HBM: many frameless blocks per zxc_b200_compress_blocks_device / zxc_b200_decompress_blocks_device call.  Kept
-apart from ``zxc_b200`` so that importing the package does not import torch.
+API in HBM: many frameless blocks per zxc_b200_compress_blocks_device / zxc_b200_decompress_blocks_device call.
+``DeviceDict`` prepares a dictionary in HBM once; passed as ``dict`` to those helpers it makes them call the _using_dict
+entry points, which stage nothing per call.  Kept apart from ``zxc_b200`` so that importing the package does not
+import torch.
 """
 import ctypes as C
 import warnings
@@ -67,6 +69,92 @@ class ZxcError(RuntimeError):
         self.code = int(code)
 
 
+lib.zxc_b200_dict_device_create.restype = C.c_void_p
+lib.zxc_b200_dict_device_create.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
+lib.zxc_b200_dict_device_id.restype = C.c_uint32
+lib.zxc_b200_dict_device_id.argtypes = [C.c_void_p]
+lib.zxc_b200_dict_device_size.restype = C.c_size_t
+lib.zxc_b200_dict_device_size.argtypes = [C.c_void_p]
+lib.zxc_b200_dict_device_free.restype = None
+lib.zxc_b200_dict_device_free.argtypes = [C.c_void_p]
+
+
+class DeviceDict:
+    """A dictionary prepared once in HBM (zxc_b200_dict_device_create) on the current CUDA device, to which it is
+    bound.  Pass it as `dict` to the helpers below: they then call the _using_dict entry points, which stage nothing
+    per call.  The host bytes are kept (.dict, .dict_huf), so a DeviceFrame made with it can still be decoded by
+    `decompress`.  Raises ZxcError with zxc_b200_dict_device_create's code when it returns NULL."""
+
+    def __init__(self, dict, dict_huf=None, stream=None):
+        self._h = None  # before any check: __del__ runs on a half-made object too
+        self.dict = bytes(dict)
+        self.dict_huf = bytes(dict_huf) if dict_huf is not None else None
+        self.device = torch.device("cuda", torch.cuda.current_device())
+        err = C.c_int(0)
+        with torch.cuda.device(self.device):
+            stream = stream or torch.cuda.current_stream(self.device)
+            h = lib.zxc_b200_dict_device_create(self.dict, len(self.dict), self.dict_huf, C.byref(err),
+                                                stream.cuda_stream)
+        if not h:
+            raise ZxcError(err.value, "zxc_b200_dict_device_create")
+        self._h = h
+
+    @property
+    def id(self):
+        return int(lib.zxc_b200_dict_device_id(self.handle))
+
+    @property
+    def size(self):
+        return int(lib.zxc_b200_dict_device_size(self.handle))
+
+    @property
+    def handle(self):
+        if self._h is None:
+            raise ValueError("DeviceDict is closed")
+        return self._h
+
+    def close(self):
+        """Frees the device copy (after the work in flight on its device); later use raises ValueError."""
+        if self._h is not None:
+            lib.zxc_b200_dict_device_free(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        self.close()
+
+
+def _dict_opts(o, dict, dict_huf):
+    """Puts host dictionary bytes into the options o; returns (the bytes to keep alive, None).  For a DeviceDict, leaves
+    o without a dictionary and returns ([], the DeviceDict)."""
+    if isinstance(dict, DeviceDict):
+        if dict_huf is not None:
+            raise ValueError("dict_huf goes into DeviceDict(dict, dict_huf), not beside it")
+        return [], dict
+    keep = []
+    if dict is not None:
+        d = bytes(dict)
+        keep.append(d)
+        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+        if dict_huf is not None:
+            h = bytes(dict_huf)
+            keep.append(h)
+            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    return keep, None
+
+
+def _call(name, dd, head, tail):
+    """lib.name(*head, *tail), or with a DeviceDict its _using_dict variant, which takes the handle between the two"""
+    if dd is None:
+        return getattr(lib, name)(*head, *tail)
+    return getattr(lib, name + "_using_dict")(*head, dd.handle, *tail)
+
+
 @dataclass
 class DeviceFrame:
     frame: torch.Tensor  # uint8, the complete frame (a view of the compress buffer, trimmed to the frame size)
@@ -94,20 +182,13 @@ def compress(src, *, level=0, block_size=0, checksum=False, seekable=False, dict
     """Compress a contiguous CUDA tensor (its bytes) into a ZXC frame on its device; returns a DeviceFrame.
 
     Runs on `stream` (default: torch's current stream of src's device) and synchronises it once to read the frame
-    size.  The frame equals what zxc_compress returns for the same bytes and options."""
+    size.  The frame equals what zxc_compress returns for the same bytes and options.  dict / dict_huf are host bytes,
+    or dict is a DeviceDict (zxc_b200_compress_device_using_dict: nothing is staged)."""
     b = _bytes_view(src)
     n = b.numel()
     bs = block_size or BLOCK_SIZE_DEFAULT
-    keep = []
     o = _Opts(level=level, block_size=block_size, checksum_enabled=int(bool(checksum)), seekable=int(bool(seekable)))
-    if dict is not None:
-        d = bytes(dict)
-        keep.append(d)
-        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
-        if dict_huf is not None:
-            h = bytes(dict_huf)
-            keep.append(h)
-            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    keep, dd = _dict_opts(o, dict, dict_huf)
     with torch.cuda.device(b.device):
         stream = stream or torch.cuda.current_stream(b.device)
         with torch.cuda.stream(stream):
@@ -120,15 +201,17 @@ def compress(src, *, level=0, block_size=0, checksum=False, seekable=False, dict
             result = torch.empty(1, dtype=torch.int64, device=b.device)
             n_blocks = (n + bs - 1) // bs
             jobs = torch.empty(max(n_blocks, 1) * JOB_BYTES, dtype=torch.uint8, device=b.device)[: n_blocks * JOB_BYTES]
-            rc = lib.zxc_b200_compress_device(b.data_ptr() if n else None, n, dst.data_ptr(), cap, C.byref(o),
-                                              scratch.data_ptr(), scratch_size, result.data_ptr(),
-                                              jobs.data_ptr() if n_blocks else None, stream.cuda_stream)
+            rc = _call("zxc_b200_compress_device", dd, (b.data_ptr() if n else None, n, dst.data_ptr(), cap, C.byref(o)),
+                       (scratch.data_ptr(), scratch_size, result.data_ptr(), jobs.data_ptr() if n_blocks else None,
+                        stream.cuda_stream))
             if rc != 0:
                 raise ZxcError(rc, "zxc_b200_compress_device")
             stream.synchronize()
             size = int(result.item())
     if size < 0:
         raise ZxcError(size, "zxc_b200_compress_device")
+    if dd is not None:  # the handle keeps its host bytes, so decompress can stage them
+        return DeviceFrame(dst[:size], jobs, bs, n, bool(checksum), dd.dict, dd.dict_huf)
     return DeviceFrame(dst[:size], jobs, bs, n, bool(checksum), keep[0] if dict is not None else None,
                        keep[1] if dict_huf is not None and dict is not None else None)
 
@@ -180,21 +263,13 @@ def decompress_frame(frame, *, capacity=None, dict=None, dict_huf=None, checksum
     block_size per 8 bytes of frame); a footer past that raises ValueError, and a large plausible one can still ask
     for more device memory than there is (torch's OutOfMemoryError).  For frames from an untrusted source pass
     capacity: the output room to allow.  checksum=True verifies the block
-    checksums and the global hash when the frame has them.  dict / dict_huf are host bytes."""
+    checksums and the global hash when the frame has them.  dict / dict_huf are host bytes, or dict is a DeviceDict."""
     if not frame.is_cuda or frame.dtype != torch.uint8 or not frame.is_contiguous():
         raise ValueError("frame must be a contiguous uint8 CUDA tensor")
     f = frame.reshape(-1)
     n = f.numel()
     o = _DOpts(checksum_enabled=int(bool(checksum)))
-    keep = []
-    if dict is not None:
-        d = bytes(dict)
-        keep.append(d)
-        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
-        if dict_huf is not None:
-            h = bytes(dict_huf)
-            keep.append(h)
-            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    keep, dd = _dict_opts(o, dict, dict_huf)
     dev = f.device
     with torch.cuda.device(dev):
         stream = stream or torch.cuda.current_stream(dev)
@@ -215,9 +290,9 @@ def decompress_frame(frame, *, capacity=None, dict=None, dict_huf=None, checksum
             out = torch.empty(max(capacity, 1), dtype=torch.uint8, device=dev)
             scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
             result = torch.empty(1, dtype=torch.int64, device=dev)
-            rc = lib.zxc_b200_decompress_device(f.data_ptr(), n, out.data_ptr() if capacity else None, capacity,
-                                                C.byref(o), scratch.data_ptr(), scratch_size, result.data_ptr(),
-                                                stream.cuda_stream)
+            rc = _call("zxc_b200_decompress_device", dd,
+                       (f.data_ptr(), n, out.data_ptr() if capacity else None, capacity, C.byref(o)),
+                       (scratch.data_ptr(), scratch_size, result.data_ptr(), stream.cuda_stream))
             if rc != 0:
                 raise ZxcError(rc, "zxc_b200_decompress_device")
             stream.synchronize()
@@ -273,21 +348,13 @@ def decompress_inplace(buf, comp_size, *, dict=None, dict_huf=None, checksum=Fal
     the round schedule, which leaves it as it was).  `window` is the compressed bytes staged per round, default
     min(comp_size, 256 MiB); a window of comp_size decodes in one round unless the scratch it takes reads as one for a
     larger block size (see zxc_b200_decompress_inplace_device in zxc_b200.h).  Reads the frame's header byte that
-    sizes the scratch with one small copy.  dict / dict_huf are host bytes."""
+    sizes the scratch with one small copy.  dict / dict_huf are host bytes, or dict is a DeviceDict."""
     if not buf.is_cuda or buf.dtype != torch.uint8 or not buf.is_contiguous():
         raise ValueError("buf must be a contiguous uint8 CUDA tensor")
     b = buf.reshape(-1)
     cap, comp_size = b.numel(), int(comp_size)
     o = _DOpts(checksum_enabled=int(bool(checksum)))
-    keep = []
-    if dict is not None:
-        d = bytes(dict)
-        keep.append(d)
-        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
-        if dict_huf is not None:
-            h = bytes(dict_huf)
-            keep.append(h)
-            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    keep, dd = _dict_opts(o, dict, dict_huf)
     window = min(int(window) if window is not None else WINDOW_DEFAULT, comp_size)
     dev = b.device
     with torch.cuda.device(dev):
@@ -302,8 +369,8 @@ def decompress_inplace(buf, comp_size, *, dict=None, dict_huf=None, checksum=Fal
                 raise ValueError("zxc_b200_decompress_inplace_device_scratch_size: buffer too large, or no device")
             scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
             result = torch.empty(1, dtype=torch.int64, device=dev)
-            rc = lib.zxc_b200_decompress_inplace_device(b.data_ptr(), cap, comp_size, C.byref(o), scratch.data_ptr(),
-                                                        scratch_size, result.data_ptr(), stream.cuda_stream)
+            rc = _call("zxc_b200_decompress_inplace_device", dd, (b.data_ptr(), cap, comp_size, C.byref(o)),
+                       (scratch.data_ptr(), scratch_size, result.data_ptr(), stream.cuda_stream))
             if rc != 0:
                 raise ZxcError(rc, "zxc_b200_decompress_inplace_device")
             stream.synchronize()
@@ -356,7 +423,7 @@ def decompress_frames(frames, capacities=None, *, out=None, dict=None, dict_huf=
     zxc_b200_decompress_device with a scratch sized for it gives): by default the largest any frame's header names
     when capacities are read from the footers, else 64 KiB.  The work runs on `stream` (default: the current stream), which first waits for the current stream; with `out` or
     capacities given nothing synchronises.  Argument errors raise ValueError before anything is enqueued; a rejected
-    call raises ZxcError.  dict / dict_huf are host bytes, one dictionary for the batch."""
+    call raises ZxcError.  dict / dict_huf are host bytes, one dictionary for the batch, or dict is a DeviceDict."""
     frames = list(frames)
     if not frames:
         raise ValueError("frames is empty")
@@ -387,15 +454,7 @@ def decompress_frames(frames, capacities=None, *, out=None, dict=None, dict_huf=
         if any(c < 0 for c in capacities):
             raise ValueError("capacities must not be negative")
     o = _DOpts(checksum_enabled=int(bool(checksum)))
-    keep = []
-    if dict is not None:
-        d = bytes(dict)
-        keep.append(d)
-        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
-        if dict_huf is not None:
-            h = bytes(dict_huf)
-            keep.append(h)
-            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    keep, dd = _dict_opts(o, dict, dict_huf)
     with torch.cuda.device(dev):
         current = torch.cuda.current_stream(dev)
         stream = stream or current
@@ -432,8 +491,8 @@ def decompress_frames(frames, capacities=None, *, out=None, dict=None, dict_huf=
                 raise ValueError("zxc_b200_decompress_device_batch_scratch_size: too many frames or bytes, or no device")
             scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
             results = torch.empty(n, dtype=torch.int64, device=dev)
-            rc = lib.zxc_b200_decompress_device_batch(desc.data_ptr(), n, C.byref(o), scratch.data_ptr(),
-                                                      scratch_size, results.data_ptr(), stream.cuda_stream)
+            rc = _call("zxc_b200_decompress_device_batch", dd, (desc.data_ptr(), n, C.byref(o)),
+                       (scratch.data_ptr(), scratch_size, results.data_ptr(), stream.cuda_stream))
             if rc != 0:
                 raise ZxcError(rc, "zxc_b200_decompress_device_batch")
     return out, results
@@ -456,7 +515,7 @@ def compress_frames(srcs, *, level=0, block_size=0, checksum=False, seekable=Fal
     contiguous uint8 tensors on the inputs' device, one per input, takes the frames instead.  The work runs on `stream`
     (default: the current stream), which first waits for the current stream; nothing synchronises.  Argument errors
     raise ValueError before anything is enqueued; a rejected call raises ZxcError with its code.  dict / dict_huf are
-    host bytes, one dictionary for the batch."""
+    host bytes, one dictionary for the batch, or dict is a DeviceDict."""
     srcs = list(srcs)
     if not srcs:
         raise ValueError("srcs is empty")
@@ -475,15 +534,7 @@ def compress_frames(srcs, *, level=0, block_size=0, checksum=False, seekable=Fal
         for o in out:
             _check_out(o, dev)
     o = _Opts(level=level, block_size=block_size, checksum_enabled=int(bool(checksum)), seekable=int(bool(seekable)))
-    keep = []
-    if dict is not None:
-        d = bytes(dict)
-        keep.append(d)
-        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
-        if dict_huf is not None:
-            h = bytes(dict_huf)
-            keep.append(h)
-            o.dict_huf = C.cast(C.c_char_p(h), C.c_void_p)
+    keep, dd = _dict_opts(o, dict, dict_huf)
     # 0 for options the call rejects (it then gives their exact code below with a token scratch), or a batch too large
     scratch_size = int(lib.zxc_b200_compress_device_batch_scratch_size(n, sum(t.numel() for t in srcs), C.byref(o)))
     with torch.cuda.device(dev):
@@ -503,8 +554,8 @@ def compress_frames(srcs, *, level=0, block_size=0, checksum=False, seekable=Fal
             desc = desc.pin_memory().to(dev, non_blocking=True)
             scratch = torch.empty(max(scratch_size, 1), dtype=torch.uint8, device=dev)
             results = torch.empty(n, dtype=torch.int64, device=dev)
-            rc = lib.zxc_b200_compress_device_batch(desc.data_ptr(), n, C.byref(o), scratch.data_ptr(), scratch_size,
-                                                    results.data_ptr(), stream.cuda_stream)
+            rc = _call("zxc_b200_compress_device_batch", dd, (desc.data_ptr(), n, C.byref(o)),
+                       (scratch.data_ptr(), scratch_size, results.data_ptr(), stream.cuda_stream))
             if rc != 0:
                 raise ZxcError(rc, "zxc_b200_compress_device_batch")
     return out, results
@@ -522,6 +573,14 @@ lib.zxc_b200_decompress_blocks_device_scratch_size.argtypes = [C.c_uint32, C.c_u
 lib.zxc_b200_decompress_blocks_device.restype = C.c_int
 lib.zxc_b200_decompress_blocks_device.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_int, C.c_void_p, C.c_size_t,
                                                   C.c_void_p, C.c_void_p]
+# the _using_dict variants: the base call's arguments with the DeviceDict handle right after opts
+for _name, _opts_at in (("compress_device", 4), ("compress_device_batch", 2), ("compress_blocks_device", 2),
+                        ("decompress_device", 4), ("decompress_inplace_device", 3), ("decompress_device_batch", 2),
+                        ("decompress_blocks_device", 2)):
+    _base = getattr(lib, f"zxc_b200_{_name}")
+    _var = getattr(lib, f"zxc_b200_{_name}_using_dict")
+    _var.restype = C.c_int
+    _var.argtypes = _base.argtypes[: _opts_at + 1] + [C.c_void_p] + _base.argtypes[_opts_at + 1:]
 
 
 def _same_device(tensors, what):
@@ -567,7 +626,7 @@ def compress_blocks(srcs, *, level=0, checksum=False, dict=None, out=None, strea
     zxc_compress_block_bound(len) bytes by default; `out`, a list of contiguous uint8 tensors on the inputs' device,
     one per input, takes the blocks instead.  The work runs on `stream` (default: the current stream), which first
     waits for the current stream; nothing synchronises.  Argument errors raise ValueError before anything is enqueued;
-    a rejected call raises ZxcError.  dict is host bytes, one dictionary for the batch."""
+    a rejected call raises ZxcError.  dict is host bytes, one dictionary for the batch, or a DeviceDict."""
     srcs, dev = _same_device(srcs, "srcs")
     if out is not None:
         out = list(out)
@@ -576,11 +635,7 @@ def compress_blocks(srcs, *, level=0, checksum=False, dict=None, out=None, strea
         for o in out:
             _check_out(o, dev)
     o = _Opts(level=level, checksum_enabled=int(bool(checksum)))
-    keep = []
-    if dict is not None:
-        d = bytes(dict)
-        keep.append(d)
-        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+    keep, dd = _dict_opts(o, dict, None)
     sizes = [t.numel() for t in srcs]
     # 0 for a batch the call cannot plan (it then gives its exact code with a token scratch)
     scratch_size = int(lib.zxc_b200_compress_blocks_device_scratch_size(len(srcs), sum(sizes),
@@ -591,8 +646,8 @@ def compress_blocks(srcs, *, level=0, checksum=False, dict=None, out=None, strea
 
     def call(desc, results, stream):
         scratch = torch.empty(max(scratch_size, 1), dtype=torch.uint8, device=dev)
-        rc = lib.zxc_b200_compress_blocks_device(desc.data_ptr(), len(srcs), C.byref(o), scratch.data_ptr(),
-                                                 scratch_size, results.data_ptr(), stream.cuda_stream)
+        rc = _call("zxc_b200_compress_blocks_device", dd, (desc.data_ptr(), len(srcs), C.byref(o)),
+                   (scratch.data_ptr(), scratch_size, results.data_ptr(), stream.cuda_stream))
         if rc != 0:
             raise ZxcError(rc, "zxc_b200_compress_blocks_device")
 
@@ -608,7 +663,8 @@ def decompress_blocks(blocks, sizes, *, safe=False, checksum=False, dict=None, o
     (the bytes are outs[i][:results[i]]) or a negative zxc_error_t code.  `out`, a list of contiguous uint8 tensors on
     the blocks' device, one per block, takes the outputs instead (its sizes must equal sizes).  The work runs on
     `stream` (default: the current stream), which first waits for the current stream; nothing synchronises.  Argument
-    errors raise ValueError before anything is enqueued; a rejected call raises ZxcError.  dict is host bytes."""
+    errors raise ValueError before anything is enqueued; a rejected call raises ZxcError.  dict is host bytes or a
+    DeviceDict."""
     blocks, dev = _same_device(blocks, "blocks")
     sizes = [int(c) for c in sizes]
     if len(sizes) != len(blocks):
@@ -624,11 +680,7 @@ def decompress_blocks(blocks, sizes, *, safe=False, checksum=False, dict=None, o
         if [o.numel() for o in out] != sizes:
             raise ValueError("sizes differ from the sizes of out")
     o = _DOpts(checksum_enabled=int(bool(checksum)))
-    keep = []
-    if dict is not None:
-        d = bytes(dict)
-        keep.append(d)
-        o.dict, o.dict_size = C.cast(C.c_char_p(d), C.c_void_p), len(d)
+    keep, dd = _dict_opts(o, dict, None)
     scratch_size = int(lib.zxc_b200_decompress_blocks_device_scratch_size(len(blocks), max(sizes)))
     if scratch_size == 0:
         raise ValueError("zxc_b200_decompress_blocks_device_scratch_size: too many blocks, or no device")
@@ -637,9 +689,8 @@ def decompress_blocks(blocks, sizes, *, safe=False, checksum=False, dict=None, o
 
     def call(desc, results, stream):
         scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
-        rc = lib.zxc_b200_decompress_blocks_device(desc.data_ptr(), len(blocks), C.byref(o), int(bool(safe)),
-                                                   scratch.data_ptr(), scratch_size, results.data_ptr(),
-                                                   stream.cuda_stream)
+        rc = _call("zxc_b200_decompress_blocks_device", dd, (desc.data_ptr(), len(blocks), C.byref(o)),
+                   (int(bool(safe)), scratch.data_ptr(), scratch_size, results.data_ptr(), stream.cuda_stream))
         if rc != 0:
             raise ZxcError(rc, "zxc_b200_decompress_blocks_device")
 
