@@ -613,6 +613,35 @@ ZXC_EXPORT size_t zxc_b200_dstream_device_in_size(const zxc_b200_dstream_device*
 ZXC_EXPORT size_t zxc_b200_dstream_device_out_size(const zxc_b200_dstream_device* ds);
 ZXC_EXPORT void zxc_b200_dstream_device_free(zxc_b200_dstream_device* ds);
 
+/* ---- dictionary training on samples in HBM: the device twins of zxc_train_dict, zxc_train_dict_huf and
+ *      zxc_dict_train (include/zxc_dict.h) ---- */
+/* Each takes its host trainer's arguments plus `stream`, and the one difference is where the sample bytes are:
+ *   - samples and sample_sizes are HOST arrays of n_samples entries; each samples[i] is a device pointer on the current
+ *     CUDA device, with any alignment; samples may repeat or overlap.  dict, dict_buf, huf_lengths_out and zxd_buf are
+ *     host memory, as for the host trainers.
+ *   - For every argument, the return value and the bytes written equal what this library's host trainer gives for host
+ *     copies of the same samples (and so the reference's, wherever the host trainers equal it).  That includes the
+ *     verdicts and their order: ZXC_ERROR_NULL_INPUT, ZXC_ERROR_DICT_TOO_LARGE, ZXC_ERROR_SRC_TOO_SMALL, then
+ *     ZXC_B200_ERROR_NO_DEVICE, all made before any sample byte is read.  A NULL sample of non-zero size reads as zeros
+ *     in the content trainer and is skipped by the table trainer, as the host trainers do.
+ *   - Reads: only samples[i][0 .. sample_sizes[i]) of device memory.  Nothing in device memory is written but the
+ *     library's own buffers.
+ *   - Synchronous and ordered on `stream` (a cudaStream_t, NULL = legacy default stream): the call's work follows what
+ *     is already enqueued on `stream` (a sample a kernel just wrote there is seen), and the call returns once its work
+ *     is complete.  Not capturable in a CUDA graph.  Calls on separate threads may run at once.
+ *   - Work per call, whatever n_samples: the host trainer's launches and copies plus one gather kernel
+ *     (zxc_b200_launch_count) whenever the trainer has sample bytes to gather, so zxc_b200_dict_train_device launches
+ *     two more than zxc_dict_train; the gather's piece table (24 bytes per sample, or per 64 KiB of a larger one) is
+ *     one host-to-device copy.  No sample byte crosses PCIe.
+ *   - zxc_b200_train_phase_times fills the same slots; its upload slots time the piece-table copy and the gather. */
+ZXC_EXPORT int64_t zxc_b200_train_dict_device(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
+                                              void* dict_buf, size_t dict_capacity, void* stream);
+ZXC_EXPORT int zxc_b200_train_dict_huf_device(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
+                                              const void* dict, size_t dict_size, uint8_t* huf_lengths_out,
+                                              void* stream);
+ZXC_EXPORT int64_t zxc_b200_dict_train_device(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
+                                              void* zxd_buf, size_t zxd_capacity, void* stream);
+
 /* Kernels launched by this library since load (for bench.py's gpu_launches). */
 ZXC_EXPORT uint64_t zxc_b200_launch_count(void);
 
@@ -622,7 +651,7 @@ ZXC_EXPORT int zxc_b200_decode_occupancy(int* lean, int* general);
 
 /* Phase times (ms) of the calling thread's last dictionary-training calls, for profiles/train_bench.py: upload,
  * count, segments, host sort, pick (zxc_train_dict); slice upload, histogram encode, code lengths
- * (zxc_train_dict_huf).  Writes min(n, 8) entries and returns their number. */
+ * (zxc_train_dict_huf); the device twins fill the same slots.  Writes min(n, 8) entries and returns their number. */
 ZXC_EXPORT int zxc_b200_train_phase_times(double* ms, int n);
 
 #ifdef __cplusplus

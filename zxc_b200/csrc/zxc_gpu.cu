@@ -2551,6 +2551,59 @@ static void tev_free(train_events* T) {
     for (int i = 0; i < T->n; i++) cudaEventDestroy(T->ev[i]);
 }
 
+/* Packs n device pieces back to back into d_dst in one zxc_ps_gather launch (none when they hold no bytes).  The host
+ * cuts every piece into parts of at most ZXG_PS_PIECE bytes and uploads that table into ZXG_BUF_OUT, which no trainer
+ * uses otherwise.  A NULL piece of non-zero size reads as zeros. */
+static int d2d_gather(zxg_ctx* c, u8* d_dst, const void* const* pieces, const size_t* sizes, size_t n) {
+    size_t m = 0;
+    for (size_t i = 0; i < n; i++) m += (sizes[i] + ZXG_PS_PIECE - 1) / ZXG_PS_PIECE;
+    if (m == 0) return ZXC_OK;
+    if (m > UINT32_MAX) return ZXC_ERROR_MEMORY;
+    zxg_psseg_t* h = (zxg_psseg_t*)malloc(m * sizeof *h);
+    zxg_psseg_t* d = (zxg_psseg_t*)zxg_buffer(c, ZXG_BUF_OUT, m * sizeof *h);
+    if (!h || !d) {
+        free(h);
+        return ZXC_ERROR_MEMORY;
+    }
+    u64 off = 0;
+    size_t k = 0;
+    for (size_t i = 0; i < n; i++) {
+        const u64 s = (u64)(uintptr_t)pieces[i];
+        for (u64 o = 0; o < sizes[i]; o += ZXG_PS_PIECE, k++) {
+            h[k].src = s ? s + o : 0;
+            h[k].dst = (u64)(uintptr_t)(d_dst + off + o);
+            h[k].len = sizes[i] - o < ZXG_PS_PIECE ? sizes[i] - o : ZXG_PS_PIECE;
+        }
+        off += sizes[i];
+    }
+    int rc = zxg_h2d(c, d, h, m * sizeof *h); /* the host table has been read when it returns */
+    free(h);
+    if (rc != ZXC_OK) return rc;
+    const u32 gmax = (u32)(g_sm_count > 0 ? g_sm_count : 132) * 8u;
+    zxc_ps_gather<<<m < gmax ? (u32)m : gmax, 256, 0, c->stream>>>(d, (u32)m);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* Fills d_dst with the samples, packed: from host memory through the bounce buffers, or, for device samples, after the
+ * work enqueued on the caller's stream (an event orders the context's stream behind it) by d2d_gather.  T->ev[0] is
+ * recorded once the context's stream may start, so the upload slot times the transfer alone. */
+static int gather_samples(zxg_ctx* c, u8* d_dst, const void* const* pieces, const size_t* sizes, size_t n,
+                          const zxg_train_src_t* src, train_events* T) {
+    if (src && src->device) {
+        cudaEvent_t ev;
+        if (cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+        const bool ok = cudaEventRecord(ev, (cudaStream_t)src->stream) == cudaSuccess &&
+                        cudaStreamWaitEvent(c->stream, ev, 0) == cudaSuccess;
+        cudaEventDestroy(ev);
+        if (!ok) return ZXC_B200_ERROR_CUDA;
+        cudaEventRecord(T->ev[0], c->stream);
+        return d2d_gather(c, d_dst, pieces, sizes, n);
+    }
+    cudaEventRecord(T->ev[0], c->stream);
+    return h2d_gather(c, d_dst, pieces, sizes, n);
+}
+
 static int grid_cap(unsigned long long want, u32 per_sm) {
     const unsigned long long cap = (unsigned long long)(g_sm_count > 0 ? g_sm_count : 132) * per_sm;
     return (int)(want < 1 ? 1 : (want < cap ? want : cap));
@@ -2564,7 +2617,7 @@ static size_t trn_kept_off(u32 n_starts) { return (TRN_STARTS_OFF + (size_t)n_st
 
 extern "C" int zxg_train_segments(zxg_ctx* c, const void* const* samples, const size_t* sizes, size_t n_samples,
                                   uint64_t corpus_size, uint64_t freq_stride, uint64_t seg_stride, uint32_t n_starts,
-                                  uint32_t seg_alloc, zxg_seg_t* h_segs, uint32_t* n_segs) {
+                                  uint32_t seg_alloc, zxg_seg_t* h_segs, uint32_t* n_segs, const zxg_train_src_t* src) {
     *n_segs = 0;
     u8* d_corpus = (u8*)zxg_buffer(c, ZXG_BUF_IN, (size_t)corpus_size + 16);
     u8* aux = (u8*)zxg_buffer(c, ZXG_BUF_AUX, trn_kept_off(n_starts) + (size_t)seg_alloc * sizeof(TrainSeg) + 256);
@@ -2575,10 +2628,7 @@ extern "C" int zxg_train_segments(zxg_ctx* c, const void* const* samples, const 
     TrainSeg* d_kept = (TrainSeg*)(aux + trn_kept_off(n_starts));
     train_events T;
     int rc = tev_init(&T, 4);
-    if (rc == ZXC_OK) {
-        cudaEventRecord(T.ev[0], c->stream);
-        rc = h2d_gather(c, d_corpus, samples, sizes, n_samples);
-    }
+    if (rc == ZXC_OK) rc = gather_samples(c, d_corpus, samples, sizes, n_samples, src, &T);
     if (rc == ZXC_OK && (cudaMemsetAsync(d_corpus + corpus_size, 0, 16, c->stream) != cudaSuccess ||
                          cudaMemsetAsync(d_freq, 0, TRN_RES_OFF + 256, c->stream) != cudaSuccess))
         rc = ZXC_B200_ERROR_CUDA;
@@ -2704,7 +2754,7 @@ extern "C" int zxg_train_tail(zxg_ctx* c, uint64_t corpus_size, uint32_t bytes, 
 }
 
 extern "C" int zxg_train_literals(zxg_ctx* c, const void* const* pieces, const size_t* sizes, size_t n, const void* h_dict,
-                                  uint32_t dict_size, uint32_t* h_freq) {
+                                  uint32_t dict_size, uint32_t* h_freq, const zxg_train_src_t* src) {
     memset(h_freq, 0, 256 * sizeof(uint32_t));
     if (n == 0) return ZXC_OK;
     const u32 bs = 4096u, level = 6u; /* the reference trains at ZXC_LEVEL_DENSITY on 4 KiB slices */
@@ -2732,10 +2782,7 @@ extern "C" int zxg_train_literals(zxg_ctx* c, const void* const* pieces, const s
     }
     train_events T;
     int rc = tev_init(&T, 3);
-    if (rc == ZXC_OK) {
-        cudaEventRecord(T.ev[0], c->stream);
-        rc = h2d_gather(c, d_src, pieces, sizes, n);
-    }
+    if (rc == ZXC_OK) rc = gather_samples(c, d_src, pieces, sizes, n, src, &T);
     if (rc == ZXC_OK &&
         (cudaMemsetAsync(d_src + total, 0, 64, c->stream) != cudaSuccess ||
          cudaMemcpyAsync(d_sl, h_sl, n * sizeof(TrainSlice), cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||

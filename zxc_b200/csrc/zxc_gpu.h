@@ -246,22 +246,29 @@ int zxg_decode_staged(zxg_ctx* c, const uint8_t* h_src, zxg_fetch_fn fetch, void
  * The content trainer runs zxg_train_segments, orders the segments on the host, then zxg_train_pick (or
  * zxg_train_tail) on the same context: the corpus and the k-gram table stay on the device in between. */
 typedef struct { uint32_t offset, len, score; } zxg_seg_t; /* len 0: no segment */
+/* Where the samples are: host memory (NULL, or device == 0), or device memory on the current device, read after the
+ * work enqueued on `stream` (a cudaStream_t) so far. */
+typedef struct {
+    int device;
+    void* stream;
+} zxg_train_src_t;
 
-/* Uploads the samples as one corpus, counts the k-grams at every freq_stride-th position, builds a segment per
+/* Packs the samples into one device corpus, counts the k-grams at every freq_stride-th position, builds a segment per
  * start (start s at s * seg_stride, n_starts of them) and keeps the first seg_alloc in position order:
  * h_segs (seg_alloc entries) and *n_segs. */
 int zxg_train_segments(zxg_ctx* c, const void* const* samples, const size_t* sizes, size_t n_samples,
                        uint64_t corpus_size, uint64_t freq_stride, uint64_t seg_stride, uint32_t n_starts,
-                       uint32_t seg_alloc, zxg_seg_t* h_segs, uint32_t* n_segs);
+                       uint32_t seg_alloc, zxg_seg_t* h_segs, uint32_t* n_segs, const zxg_train_src_t* src);
 /* The greedy pick over the segments in the given order and the reversed emission into h_out (capacity bytes);
  * *filled = bytes picked (0: nothing selected). */
 int zxg_train_pick(zxg_ctx* c, uint64_t corpus_size, const zxg_seg_t* h_sorted, uint32_t n_segs, uint32_t capacity,
                    uint8_t* h_out, uint32_t* filled);
 /* The last `bytes` bytes of the uploaded corpus. */
 int zxg_train_tail(zxg_ctx* c, uint64_t corpus_size, uint32_t bytes, uint8_t* h_out);
-/* Literal histogram (256 counts) of the level-6 parses of [dict | piece] for every piece (<= 4096 bytes each). */
+/* Literal histogram (256 counts) of the level-6 parses of [dict | piece] for every piece (<= 4096 bytes each), the
+ * pieces packed as the samples of zxg_train_segments are. */
 int zxg_train_literals(zxg_ctx* c, const void* const* pieces, const size_t* sizes, size_t n, const void* h_dict,
-                       uint32_t dict_size, uint32_t* h_freq);
+                       uint32_t dict_size, uint32_t* h_freq, const zxg_train_src_t* src);
 
 /* Phase times (ms) of the calling thread's last training calls: device time from CUDA events, host time from the
  * host clock. */

@@ -61,8 +61,10 @@ static void seg_sort_desc(zxg_seg_t* a, size_t n) {
     }
 }
 
-int64_t zxc_train_dict(const void* const* samples, const size_t* sample_sizes, size_t n_samples, void* dict_buf,
-                       size_t dict_capacity) {
+/* The bodies of the trainers and of their device twins: `src` says where the sample bytes are.  Everything before
+ * the gather -- verdicts, sampling arithmetic, which slices are kept -- is the same code for both. */
+static int64_t train_dict(const void* const* samples, const size_t* sample_sizes, size_t n_samples, void* dict_buf,
+                          size_t dict_capacity, const zxg_train_src_t* src) {
     if (!samples || !sample_sizes || n_samples == 0 || !dict_buf || dict_capacity == 0) return ZXC_ERROR_NULL_INPUT;
     if (dict_capacity > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
     uint64_t corpus_size = 0;
@@ -95,7 +97,7 @@ int64_t zxc_train_dict(const void* const* samples, const size_t* sample_sizes, s
     const uint32_t cap = (uint32_t)dict_capacity;
     uint32_t n_segs = 0, filled = 0;
     int rc = zxg_train_segments(g, samples, sample_sizes, n_samples, corpus_size, freq_stride, stride, n_starts, seg_alloc,
-                                segs, &n_segs);
+                                segs, &n_segs, src);
     if (rc == ZXC_OK && n_segs > 0) {
         const double t0 = now_ms();
         seg_sort_desc(segs, n_segs);
@@ -112,8 +114,8 @@ int64_t zxc_train_dict(const void* const* samples, const size_t* sample_sizes, s
     return rc != ZXC_OK ? rc : (int64_t)filled;
 }
 
-int zxc_train_dict_huf(const void* const* samples, const size_t* sample_sizes, size_t n_samples, const void* dict,
-                       size_t dict_size, uint8_t* huf_lengths_out) {
+static int train_dict_huf(const void* const* samples, const size_t* sample_sizes, size_t n_samples, const void* dict,
+                          size_t dict_size, uint8_t* huf_lengths_out, const zxg_train_src_t* src) {
     if (!samples || !sample_sizes || n_samples == 0 || !dict || dict_size == 0 || !huf_lengths_out)
         return ZXC_ERROR_NULL_INPUT;
     if (dict_size > ZXC_DICT_SIZE_MAX) return ZXC_ERROR_DICT_TOO_LARGE;
@@ -165,7 +167,7 @@ int zxc_train_dict_huf(const void* const* samples, const size_t* sample_sizes, s
     if (!g) {
         rc = ZXC_ERROR_MEMORY;
     } else {
-        rc = zxg_train_literals(g, ptrs, lens, kept, dict, (uint32_t)dict_size, freq);
+        rc = zxg_train_literals(g, ptrs, lens, kept, dict, (uint32_t)dict_size, freq, src);
         zxg_release(g);
     }
     if (rc == ZXC_OK) {
@@ -190,22 +192,56 @@ int zxc_train_dict_huf(const void* const* samples, const size_t* sample_sizes, s
     return rc;
 }
 
-int64_t zxc_dict_train(const void* const* samples, const size_t* sample_sizes, size_t n_samples, void* zxd_buf,
-                       size_t zxd_capacity) {
+static int64_t dict_train(const void* const* samples, const size_t* sample_sizes, size_t n_samples, void* zxd_buf,
+                          size_t zxd_capacity, const zxg_train_src_t* src) {
     if (!samples || !sample_sizes || n_samples == 0 || !zxd_buf || zxd_capacity == 0) return ZXC_ERROR_NULL_INPUT;
     uint8_t* content = (uint8_t*)malloc(ZXC_DICT_SIZE_MAX);
     if (!content) return ZXC_ERROR_MEMORY;
     int64_t out;
-    const int64_t content_size = zxc_train_dict(samples, sample_sizes, n_samples, content, ZXC_DICT_SIZE_MAX);
+    const int64_t content_size = train_dict(samples, sample_sizes, n_samples, content, ZXC_DICT_SIZE_MAX, src);
     if (content_size <= 0) {
         out = content_size < 0 ? content_size : ZXC_ERROR_SRC_TOO_SMALL;
     } else {
         uint8_t huf[ZXC_HUF_TABLE_SIZE];
-        const int hrc = zxc_train_dict_huf(samples, sample_sizes, n_samples, content, (size_t)content_size, huf);
+        const int hrc = train_dict_huf(samples, sample_sizes, n_samples, content, (size_t)content_size, huf, src);
         out = hrc != ZXC_OK ? hrc : zxc_dict_save(content, (size_t)content_size, huf, zxd_buf, zxd_capacity);
     }
     free(content);
     return out;
+}
+
+int64_t zxc_train_dict(const void* const* samples, const size_t* sample_sizes, size_t n_samples, void* dict_buf,
+                       size_t dict_capacity) {
+    return train_dict(samples, sample_sizes, n_samples, dict_buf, dict_capacity, NULL);
+}
+
+int zxc_train_dict_huf(const void* const* samples, const size_t* sample_sizes, size_t n_samples, const void* dict,
+                       size_t dict_size, uint8_t* huf_lengths_out) {
+    return train_dict_huf(samples, sample_sizes, n_samples, dict, dict_size, huf_lengths_out, NULL);
+}
+
+int64_t zxc_dict_train(const void* const* samples, const size_t* sample_sizes, size_t n_samples, void* zxd_buf,
+                       size_t zxd_capacity) {
+    return dict_train(samples, sample_sizes, n_samples, zxd_buf, zxd_capacity, NULL);
+}
+
+/* the device twins: the same bodies, the sample bytes gathered in HBM after the work enqueued on `stream` */
+int64_t zxc_b200_train_dict_device(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
+                                   void* dict_buf, size_t dict_capacity, void* stream) {
+    const zxg_train_src_t src = {1, stream};
+    return train_dict(samples, sample_sizes, n_samples, dict_buf, dict_capacity, &src);
+}
+
+int zxc_b200_train_dict_huf_device(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
+                                   const void* dict, size_t dict_size, uint8_t* huf_lengths_out, void* stream) {
+    const zxg_train_src_t src = {1, stream};
+    return train_dict_huf(samples, sample_sizes, n_samples, dict, dict_size, huf_lengths_out, &src);
+}
+
+int64_t zxc_b200_dict_train_device(const void* const* samples, const size_t* sample_sizes, size_t n_samples,
+                                   void* zxd_buf, size_t zxd_capacity, void* stream) {
+    const zxg_train_src_t src = {1, stream};
+    return dict_train(samples, sample_sizes, n_samples, zxd_buf, zxd_capacity, &src);
 }
 
 int zxc_b200_train_phase_times(double* ms, int n) {

@@ -11,13 +11,16 @@ into the same buffer with zxc_b200_decompress_inplace_device, and ``load_frame``
 host into HBM and expand it there with no second buffer.  ``compress_blocks`` and ``decompress_blocks`` are the block
 API in HBM: many frameless blocks per zxc_b200_compress_blocks_device / zxc_b200_decompress_blocks_device call.
 ``DeviceDict`` prepares a dictionary in HBM once; passed as ``dict`` to those helpers it makes them call the _using_dict
-entry points, which stage nothing per call.  Kept apart from ``zxc_b200`` so that importing the package does not
+entry points, which stage nothing per call.  ``train_dict``, ``train_dict_huf`` and ``dict_train`` train a dictionary on
+samples that are already in HBM (zxc_b200_train_dict_device and its siblings), and ``DeviceDict.train`` makes a
+DeviceDict from such samples.  Kept apart from ``zxc_b200`` so that importing the package does not
 import torch.
 """
 import ctypes as C
 import warnings
 from dataclasses import dataclass
 
+import numpy as np
 import torch
 
 from . import lib
@@ -113,6 +116,17 @@ class DeviceDict:
             raise ValueError("DeviceDict is closed")
         return self._h
 
+    @classmethod
+    def train(cls, samples, sizes=None, *, capacity=65535, table=True, stream=None):
+        """Trains a dictionary on samples in HBM (as train_dict, then train_dict_huf when `table`) and prepares it on
+        the samples' device: the same .id, .dict and .dict_huf as DeviceDict(zxc_train_dict(...),
+        zxc_train_dict_huf(...)) on host copies of the samples."""
+        _, _, dev = _train_samples(samples, sizes)
+        content = train_dict(samples, sizes, capacity=capacity, stream=stream)
+        huf = train_dict_huf(samples, content, sizes, stream=stream) if table else None
+        with torch.cuda.device(dev):
+            return cls(content, huf, stream=stream)
+
     def close(self):
         """Frees the device copy (after the work in flight on its device); later use raises ValueError."""
         if self._h is not None:
@@ -127,6 +141,95 @@ class DeviceDict:
 
     def __del__(self):
         self.close()
+
+
+lib.zxc_dict_save_bound.restype = C.c_size_t
+lib.zxc_dict_save_bound.argtypes = [C.c_size_t]
+lib.zxc_b200_train_dict_device.restype = C.c_int64
+lib.zxc_b200_train_dict_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+lib.zxc_b200_train_dict_huf_device.restype = C.c_int
+lib.zxc_b200_train_dict_huf_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                               C.c_void_p]
+lib.zxc_b200_dict_train_device.restype = C.c_int64
+lib.zxc_b200_dict_train_device.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
+
+
+def _train_samples(samples, sizes):
+    """The trainers' host arrays for the two sample forms: (pointers, sizes) as uint64 numpy arrays, and the device.
+    A list of uint8 CUDA tensors gives one sample per tensor; one uint8 CUDA tensor with `sizes` gives samples laid
+    back to back from its start (no sizes: the whole tensor is one sample)."""
+    def check(t):
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.uint8 or not t.is_contiguous():
+            raise ValueError("samples must be contiguous uint8 CUDA tensors")
+
+    if isinstance(samples, torch.Tensor):
+        check(samples)
+        if sizes is None:
+            sizes = [samples.numel()]
+        if isinstance(sizes, torch.Tensor):
+            sizes = sizes.cpu().numpy()
+        sz = np.asarray(sizes, dtype=np.int64).reshape(-1)
+        if (sz < 0).any():
+            raise ValueError("sizes must not be negative")
+        ends = np.cumsum(sz)
+        if sz.size and int(ends[-1]) > samples.numel():
+            raise ValueError(f"sizes add up to {int(ends[-1])} bytes, more than the tensor's {samples.numel()}")
+        ptrs = np.uint64(samples.data_ptr()) + (ends - sz).astype(np.uint64)
+        return ptrs, sz.astype(np.uint64), samples.device
+    if sizes is not None:
+        raise ValueError("sizes goes with one tensor holding the samples back to back, not with a list")
+    ts = list(samples)
+    for t in ts:
+        check(t)
+    dev = ts[0].device if ts else torch.device("cuda", torch.cuda.current_device())
+    if any(t.device != dev for t in ts):
+        raise ValueError(f"every sample must be on {dev}")
+    ptrs = np.fromiter((t.data_ptr() for t in ts), np.uint64, len(ts))
+    sz = np.fromiter((t.numel() for t in ts), np.uint64, len(ts))
+    return ptrs, sz, dev
+
+
+def _train(name, samples, sizes, stream, args):
+    """lib.name(ptrs, sizes, n, *args, stream) on `stream` (default: the current stream), which first waits for the
+    current stream; raises ZxcError for a negative result and returns it otherwise"""
+    ptrs, sz, dev = _train_samples(samples, sizes)
+    with torch.cuda.device(dev):
+        current = torch.cuda.current_stream(dev)
+        stream = stream or current
+        if stream != current:
+            stream.wait_stream(current)
+        r = int(getattr(lib, name)(ptrs.ctypes.data, sz.ctypes.data, ptrs.size, *args, stream.cuda_stream))
+    if r < 0:
+        raise ZxcError(r, name)
+    return r
+
+
+def train_dict(samples, sizes=None, *, capacity=65535, stream=None):
+    """zxc_train_dict on samples in HBM (zxc_b200_train_dict_device): the dictionary content, at most `capacity`
+    bytes, equal to what zxc_train_dict gives for host copies of the samples.  `samples` is a list of uint8 CUDA
+    tensors (views at any offset), or one uint8 CUDA tensor holding them back to back with their `sizes`.  The call is
+    synchronous on `stream` (default: the current stream, which it first waits for)."""
+    out = C.create_string_buffer(max(int(capacity), 1))
+    r = _train("zxc_b200_train_dict_device", samples, sizes, stream, (out, int(capacity)))
+    return out.raw[:r]
+
+
+def train_dict_huf(samples, dict, sizes=None, *, stream=None):
+    """zxc_train_dict_huf on samples in HBM: the 128-byte shared literal table for the dictionary content `dict`
+    (bytes), trained on the samples (as for train_dict)."""
+    d = bytes(dict)
+    huf = C.create_string_buffer(128)
+    _train("zxc_b200_train_dict_huf_device", samples, sizes, stream, (d, len(d), huf))
+    return huf.raw
+
+
+def dict_train(samples, sizes=None, *, capacity=None, stream=None):
+    """zxc_dict_train on samples in HBM: a .zxd image (content and table) of at most `capacity` bytes (default: the
+    largest a 65 535-byte content can need)."""
+    cap = int(lib.zxc_dict_save_bound(65535)) if capacity is None else int(capacity)
+    out = C.create_string_buffer(max(cap, 1))
+    r = _train("zxc_b200_dict_train_device", samples, sizes, stream, (out, cap))
+    return out.raw[:r]
 
 
 def _dict_opts(o, dict, dict_huf):
