@@ -565,6 +565,60 @@ ZXC_EXPORT int zxc_b200_seekable_device_decompress_ranges(zxc_b200_seekable_devi
                                                           size_t scratch_size, int64_t* d_results, void* stream);
 ZXC_EXPORT void zxc_b200_seekable_device_free(zxc_b200_seekable_device* h);
 
+/* ---- a SEK table for a frame in HBM: turn a frame without a table into the seekable frame, in place ---- */
+/* frame_size + zxc_seek_table_size(ceil(footer / block_size)): the buffer a frame of this size needs for
+ * zxc_b200_add_seek_table_device (frame_size itself when the footer says 0 or the frame already carries its table; 0
+ * when d_frame is NULL, frame_size is below 36, the header or footer is unreadable, the table would overflow, or there
+ * is no device).  Reads the 16 header bytes, the footer and, where a table would start, 8 bytes with up to three
+ * copies on `stream`, which it synchronises, like zxc_b200_decompress_inplace_device_bound. */
+ZXC_EXPORT uint64_t zxc_b200_seek_table_device_bound(const void* d_frame, uint64_t frame_size, void* stream);
+
+/* Scratch for zxc_b200_add_seek_table_device on frames of at most frame_size bytes and max_blocks blocks (0: no device,
+ * or more than 2^28 blocks).  About 66 bytes per block plus 1 byte per 1 024 of frame_size: a 1.8 GB frame of 65 536
+ * blocks takes 6 MB, one of a million 4 KiB blocks 70 MB.  It grows with every block, so the call finds max_blocks
+ * back from scratch_size. */
+ZXC_EXPORT size_t zxc_b200_seek_table_device_scratch_size(uint64_t frame_size, uint32_t max_blocks);
+
+/* The frame d_buffer[0 .. frame_size) (device memory) gets its SEK table, in place, on `stream`, asynchronously.
+ * On success *d_result (one device int64) is the new frame size and d_buffer[0 .. *d_result) is the frame with the
+ * table written where zxc_compress writes it: at the old footer's offset, frame_size - 12, with the footer moved
+ * behind it.  For every input and options, applying the call to zxc_compress(x) with seekable = 0 yields exactly
+ * zxc_compress(x) with seekable = 1: the file header, the blocks and the footer stay as they are, and the global hash
+ * does not cover the table.
+ * Header only: the call reads block headers, the file header and the footer.  It decodes nothing and verifies no block
+ * checksum or global hash, so a frame that gets a table may still fail to decode, with the same verdict as before.
+ * Returns ZXC_OK once enqueued, or what the host decides, in this order: ZXC_ERROR_NULL_INPUT for a NULL d_buffer,
+ * d_scratch or d_result, or frame_size > buffer_capacity (as zxc_decompress_inplace treats comp_size);
+ * ZXC_ERROR_SRC_TOO_SMALL below file header + EOF block + footer (36 bytes); ZXC_B200_ERROR_NO_DEVICE; ZXC_ERROR_MEMORY
+ * for a scratch below zxc_b200_seek_table_device_scratch_size(frame_size, 0).
+ * The device writes the rest to *d_result, in this order:
+ *   1. the file-header rejects, in zxf_read_file_header's order (those of zxc_b200_decompress_device);
+ *   2. ZXC_ERROR_BAD_HEADER wherever zxc_b200_plan_frame gives it: the sequential walk of the block headers does not
+ *      end at a valid empty EOF block;
+ *   3. ZXC_ERROR_BAD_BLOCK_TYPE for a block of the chain whose type is not RAW, GLO or GHI;
+ *   4. the tail behind the EOF block.  The footer alone goes on.  Byte for byte the table this call would write for
+ *      the chain, then the footer: the frame already has its table, the result is frame_size and nothing is written,
+ *      so applying the call twice equals applying it once.  Any other tail gives ZXC_ERROR_CORRUPT_DATA;
+ *   5. ZXC_ERROR_CORRUPT_DATA when the chain's block count N is not ceil(footer / block_size): no reader would find
+ *      such a table;
+ *   6. N = 0 gives frame_size and writes nothing (zxc_compress writes no table for an empty input);
+ *   7. ZXC_ERROR_OVERFLOW where zxc_write_seek_table gives it;
+ *   8. ZXC_ERROR_MEMORY when N exceeds the blocks the scratch was sized for.  Such a chain is not held, so its types
+ *      and sizes are not known: right after 2 it gives 5's CORRUPT_DATA, 7's OVERFLOW or this, and 3 and 4 are not
+ *      checked;
+ *   9. ZXC_ERROR_DST_TOO_SMALL when buffer_capacity < frame_size + 8 + 4 N.
+ * On a negative result, and when the result is frame_size, the buffer is left exactly as it was.  Nothing outside
+ * d_buffer[0 .. frame_size) is read, and d_buffer may have any alignment; nothing outside d_buffer[frame_size - 12 ..
+ * *d_result), the scratch and *d_result is written.  No host synchronisation and no allocation: the call may be captured
+ * in a CUDA graph, and calls on different streams with separate scratch may run at the same time.  Kernel launches per
+ * call (zxc_b200_launch_count): 43, whatever the frame.
+ * How it works (DESIGN.md section 7o): every offset whose 8 bytes could start a block of the chain is found in one
+ * parallel scan, each such candidate is linked to the one at its offset plus its on-disk size, and pointer doubling
+ * marks the chain from offset 16.  That guess is kept only when a parallel check proves that the sequential walk visits
+ * exactly those offsets; otherwise the frame is walked header by header on the device, and the walk decides. */
+ZXC_EXPORT int zxc_b200_add_seek_table_device(void* d_buffer, uint64_t frame_size, uint64_t buffer_capacity,
+                                              void* d_scratch, size_t scratch_size, int64_t* d_result, void* stream);
+
 /* ---- push streaming in HBM: the device twins of zxc_cstream_* / zxc_dstream_* (include/zxc_pstream.h) ---- */
 typedef struct zxc_b200_cstream_device_s zxc_b200_cstream_device;
 typedef struct zxc_b200_dstream_device_s zxc_b200_dstream_device;

@@ -1212,6 +1212,47 @@ size_t zxc_b200_decompress_inplace_device_bound(const void* d_src, uint64_t src_
     return inplace_bound(header, zxf_le64(footer), src_size);
 }
 
+uint64_t zxc_b200_seek_table_device_bound(const void* d_frame, uint64_t frame_size, void* stream) {
+    if (!d_frame || frame_size < ZXC_FILE_HEADER_SIZE + ZXF_BLOCK_HDR + ZXC_FILE_FOOTER_SIZE || zxg_init() != ZXC_OK)
+        return 0;
+    const uint8_t* f = (const uint8_t*)d_frame;
+    uint8_t header[ZXC_FILE_HEADER_SIZE], footer[8], sek[ZXF_BLOCK_HDR];
+    zxf_file_header_t fh;
+    if (zxg_d2h_sync(header, f, sizeof header, stream) != ZXC_OK ||
+        zxf_read_file_header(header, sizeof header, &fh, 1) != ZXC_OK ||
+        zxg_d2h_sync(footer, f + frame_size - ZXC_FILE_FOOTER_SIZE, sizeof footer, stream) != ZXC_OK)
+        return 0;
+    const uint64_t total = zxf_le64(footer);
+    if (total == 0) return frame_size;
+    const uint64_t nb = total / fh.block_size + (total % fh.block_size != 0);
+    if (nb > UINT32_MAX / ZXF_SEEK_ENTRY) return 0;
+    const uint64_t table = zxc_seek_table_size((uint32_t)nb);
+    /* the table zxw_walk's prefetch hint would find: a SEK header for nb entries where it would start */
+    if (table + ZXC_FILE_FOOTER_SIZE + ZXC_FILE_HEADER_SIZE <= frame_size) {
+        uint8_t type;
+        uint32_t comp;
+        if (zxg_d2h_sync(sek, f + frame_size - ZXC_FILE_FOOTER_SIZE - table, sizeof sek, stream) != ZXC_OK) return 0;
+        if (zxf_read_block_header(sek, sizeof sek, &type, &comp) == ZXC_OK && type == ZXF_BT_SEK &&
+            comp == (uint32_t)(nb * ZXF_SEEK_ENTRY))
+            return frame_size;
+    }
+    return frame_size + table;
+}
+
+size_t zxc_b200_seek_table_device_scratch_size(uint64_t frame_size, uint32_t max_blocks) {
+    return zxg_seek_table_scratch_bytes(frame_size, max_blocks);
+}
+
+/* The host decides what needs no frame bytes; the device decides the rest (zxc_dindex.cuh). */
+int zxc_b200_add_seek_table_device(void* d_buffer, uint64_t frame_size, uint64_t buffer_capacity, void* d_scratch,
+                                   size_t scratch_size, int64_t* d_result, void* stream) {
+    if (!d_buffer || !d_scratch || !d_result || frame_size > buffer_capacity) return ZXC_ERROR_NULL_INPUT;
+    if (frame_size < ZXC_FILE_HEADER_SIZE + ZXF_BLOCK_HDR + ZXC_FILE_FOOTER_SIZE) return ZXC_ERROR_SRC_TOO_SMALL;
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    return zxg_add_seek_table_device(d_buffer, frame_size, buffer_capacity, d_scratch, scratch_size, d_result, stream);
+}
+
 /* The host decides what zxc_decompress_inplace decides without the frame's bytes, then what
  * zxc_b200_decompress_device decides without them; the device decides the rest (zxc_dinplace.cuh). */
 static int decompress_inplace_device(void* d_buffer, uint64_t buffer_capacity, uint64_t comp_size,

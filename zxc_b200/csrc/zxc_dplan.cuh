@@ -139,6 +139,17 @@ __device__ __forceinline__ long long dp_tail(const DFrame* F, u64 produced, bool
 
 __device__ __forceinline__ void dp_prefetch(const u8* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
+/* zxf_read_file_header's rejects of the 16 header bytes at s, in its order; 1 when the header holds.  dp_probe makes
+ * the same checks inline, interleaved with its own: calling this from there changed its code generation. */
+__device__ __forceinline__ long long dp_file_header(const u8* s) {
+    if (ld32(s) != ZXF_MAGIC) return ZXC_ERROR_BAD_MAGIC;
+    if (s[4] != ZXF_VERSION) return ZXC_ERROR_BAD_VERSION;
+    if (ld16(s + 14) != dp_hash16(ld64(s), ld64(s + 8) & 0x0000FFFFFFFFFFFFull) || (s[6] & 0x0Fu) != 0)
+        return ZXC_ERROR_BAD_HEADER;
+    if (s[5] < ZXC_BLOCK_SIZE_MIN_LOG2 || s[5] > ZXC_BLOCK_SIZE_MAX_LOG2) return ZXC_ERROR_BAD_BLOCK_SIZE;
+    return 1;
+}
+
 /* the probe of frame s, of size >= header + footer, whose src_size, cap and J are set */
 __device__ __forceinline__ void dp_probe(const DDecodeOpts& o, const u8* s, DFrame* F, long long* result) {
     const u64 size = F->src_size; /* >= header + footer: checked before (on the host, or by zxc_dbatch_tiles) */

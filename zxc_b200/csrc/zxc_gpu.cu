@@ -30,6 +30,7 @@
 #include "zxc_dplan.cuh"
 #include "zxc_dinplace.cuh"
 #include "zxc_dseek.cuh"
+#include "zxc_dindex.cuh"
 #include "zxc_blocks.cuh"
 #include "zxc_pstream_device.cuh"
 #include "zxc_train.cuh"
@@ -2478,6 +2479,110 @@ extern "C" int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_
     if (rc != ZXC_OK) return rc;
     zxc_dseek_finish<<<n, DS_THREADS, 0, st>>>(A);
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* a SEK table for a device-resident frame (zxc_b200_add_seek_table_device:  */
+/* kernels in zxc_dindex.cuh)                                                */
+/* ------------------------------------------------------------------------- */
+/* Scratch layout, every region 256-aligned but the last: the state (DI_STATE_BYTES) | the scan tiles' counts (u64 per
+ * DI_TILE frame offsets) | C candidate offsets (u64) | their sizes (u32) | two jump tables (C x u32) | the marks (C
+ * bytes) | the mark tiles (u64 per ASM_TILE candidates) | the plan (J x zxc_b200_job_t), not rounded, so that the
+ * size grows with every block and the call finds J back from scratch_size.  C = 2 J + DI_C_SLACK. */
+#define DI_C_SLACK 1024u
+#define DI_J_MAX (1u << 28)
+struct DIdxLayout {
+    size_t tiles, off, len, jump[2], mark, mtiles, plan, total;
+    u32 C, J, n_tiles;
+};
+static bool di_layout(uint64_t frame_size, uint64_t J, DIdxLayout* L) {
+    const u64 scan = frame_size > ZXC_FILE_FOOTER_SIZE + ZXF_BLOCK_HDR ? frame_size - ZXC_FILE_FOOTER_SIZE - ZXF_BLOCK_HDR
+                                                                         : 1; /* offsets 0 .. the last header's */
+    const u64 n_tiles = (scan + 1 + DI_TILE - 1) / DI_TILE;
+    if (J > DI_J_MAX || n_tiles > 0x7FFFFFFFull) return false;
+    const u64 C = 2 * J + DI_C_SLACK;
+    size_t o = DI_STATE_BYTES;
+    L->tiles = o;
+    o += r256((size_t)n_tiles * 8);
+    L->off = o;
+    o += r256((size_t)C * 8);
+    L->len = o;
+    o += r256((size_t)C * 4);
+    for (int t = 0; t < 2; t++) {
+        L->jump[t] = o;
+        o += r256((size_t)C * 4);
+    }
+    L->mark = o;
+    o += r256((size_t)C);
+    L->mtiles = o;
+    o += r256((size_t)(C + ASM_TILE - 1) / ASM_TILE * 8);
+    L->plan = o;
+    o += (size_t)J * sizeof(zxc_b200_job_t);
+    L->total = o + 256; /* base alignment slack */
+    L->C = (u32)C;
+    L->J = (u32)J;
+    L->n_tiles = (u32)n_tiles;
+    return true;
+}
+
+extern "C" size_t zxg_seek_table_scratch_bytes(uint64_t frame_size, uint32_t max_blocks) {
+    if (zxg_init() != ZXC_OK) return 0;
+    DIdxLayout L;
+    return di_layout(frame_size, max_blocks, &L) ? L.total : 0;
+}
+
+/* a grid-stride kernel's CTAs for n items */
+static u32 di_grid(u64 n) {
+    const u64 g = (n + DI_THREADS - 1) / DI_THREADS;
+    return g < 1 ? 1u : (g > DI_GRID_MAX ? (u32)DI_GRID_MAX : (u32)g);
+}
+
+extern "C" int zxg_add_seek_table_device(void* d_buffer, uint64_t frame_size, uint64_t buffer_capacity,
+                                         void* d_scratch, size_t scratch_size, int64_t* d_result, void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    DIdxLayout L;
+    if (!di_layout(frame_size, 0, &L) || L.total > scratch_size) return ZXC_ERROR_MEMORY;
+    /* the largest plan whose layout fits: L.total grows with J */
+    di_layout(frame_size, largest_fit(0, DI_J_MAX, [&](u64 J) { return di_layout(frame_size, J, &L) && L.total <= scratch_size; }),
+              &L);
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    DIdxArgs A;
+    A.buf = (u8*)d_buffer;
+    A.size = frame_size;
+    A.cap = buffer_capacity;
+    A.st = (DIdxState*)base;
+    A.tiles = (unsigned long long*)(base + L.tiles);
+    A.off = (unsigned long long*)(base + L.off);
+    A.len = (unsigned int*)(base + L.len);
+    A.jump[0] = (unsigned int*)(base + L.jump[0]);
+    A.jump[1] = (unsigned int*)(base + L.jump[1]);
+    A.mark = base + L.mark;
+    A.mtiles = (unsigned long long*)(base + L.mtiles);
+    A.plan = (zxc_b200_job_t*)(base + L.plan);
+    A.result = (long long*)d_result;
+    A.C = L.C;
+    A.J = L.J;
+    A.n_tiles = L.n_tiles;
+    const u32 by_cand = di_grid(L.C), by_plan = di_grid(L.J);
+    const u32 m_tiles = (L.C + ASM_TILE - 1) / ASM_TILE;
+    zxc_dindex_probe<<<1, 1, 0, st>>>(A);
+    zxc_dindex_count<<<L.n_tiles, DI_THREADS, 0, st>>>(A);
+    zxc_dindex_tscan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_dindex_emit<<<L.n_tiles, DI_THREADS, 0, st>>>(A);
+    zxc_dindex_links<<<by_cand, DI_THREADS, 0, st>>>(A);
+    for (u32 r = 0; r < DI_ROUNDS; r++) zxc_dindex_round<<<by_cand, DI_THREADS, 0, st>>>(A, r);
+    zxc_dindex_mtiles<<<m_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dindex_mscan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+    zxc_dindex_memit<<<m_tiles, ASM_THREADS, 0, st>>>(A);
+    zxc_dindex_prove<<<by_plan, DI_THREADS, 0, st>>>(A);
+    zxc_dindex_walk<<<1, 32, 0, st>>>(A);
+    zxc_dindex_check<<<by_plan, DI_THREADS, 0, st>>>(A);
+    zxc_dindex_decide<<<1, 1, 0, st>>>(A);
+    zxc_dindex_write<<<by_plan, DI_THREADS, 0, st>>>(A);
+    __atomic_add_fetch(&g_launches, 13 + DI_ROUNDS, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }
 

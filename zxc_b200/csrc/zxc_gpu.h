@@ -173,6 +173,13 @@ size_t zxg_dseek_scratch_bytes(uint32_t block_size, uint32_t n_ranges, uint64_t 
 int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_ranges, uint32_t n_ranges, void* d_dst,
                      uint64_t dst_capacity, void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);
 
+/* A SEK table for a device-resident frame (zxc_b200_add_seek_table_device; kernels in zxc_dindex.cuh), with the
+ * arguments checked by the host.  Scratch for frames of at most frame_size bytes and max_blocks blocks (0 without a
+ * device or when that cannot be planned); ZXC_ERROR_MEMORY when the scratch holds less than that for no block. */
+size_t zxg_seek_table_scratch_bytes(uint64_t frame_size, uint32_t max_blocks);
+int zxg_add_seek_table_device(void* d_buffer, uint64_t frame_size, uint64_t buffer_capacity, void* d_scratch,
+                              size_t scratch_size, int64_t* d_result, void* stream);
+
 /* Push streams in HBM (zxc_b200_cstream_device / _dstream_device: zxc_pstream.c; kernels in zxc_pstream_device.cuh).
  * Every call enqueues on `stream`; the ones that return host values synchronise it. */
 typedef struct {

@@ -4,7 +4,8 @@
 through the host.  ``decompress`` decodes such a frame with zxc_b200_decode_blocks from the decode plan the
 compress call emitted.  ``decompress_frame`` decodes any frame held in a uint8 CUDA tensor with
 zxc_b200_decompress_device, which plans, decodes and checks it on the device.  ``SeekableFrame`` decodes byte ranges of
-a seekable frame in HBM with zxc_b200_seekable_device_decompress_ranges.  ``decompress_frames`` decodes many frames
+a seekable frame in HBM with zxc_b200_seekable_device_decompress_ranges, and ``add_seek_table`` gives a frame without a
+SEK table its table in place (zxc_b200_add_seek_table_device), so that any frame can be opened so.  ``decompress_frames`` decodes many frames
 in one zxc_b200_decompress_device_batch call, and ``compress_frames`` compresses many tensors into one frame each in
 one zxc_b200_compress_device_batch call.  ``decompress_inplace`` decodes a frame that lies flush-right in a CUDA buffer
 into the same buffer with zxc_b200_decompress_inplace_device, and ``load_frame`` uses it to bring a frame from the
@@ -828,6 +829,67 @@ def _check_out(out, device):
         raise ValueError("out must be contiguous")
     if out.device != device:
         raise ValueError(f"out must be on the frame's device {device}, not {out.device}")
+
+
+lib.zxc_b200_seek_table_device_bound.restype = C.c_uint64
+lib.zxc_b200_seek_table_device_bound.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
+lib.zxc_b200_seek_table_device_scratch_size.restype = C.c_size_t
+lib.zxc_b200_seek_table_device_scratch_size.argtypes = [C.c_uint64, C.c_uint32]
+lib.zxc_b200_add_seek_table_device.restype = C.c_int
+lib.zxc_b200_add_seek_table_device.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_size_t,
+                                               C.c_void_p, C.c_void_p]
+SEEK_TABLE_MAX_BLOCKS = 1 << 28
+
+
+def add_seek_table(frame, *, frame_size=None, stream=None):
+    """Give the ZXC frame in the first frame_size bytes (default: all) of `frame`, a contiguous uint8 CUDA tensor, its
+    SEK table; returns a uint8 tensor of the sealed frame, which SeekableFrame then opens.
+
+    Runs zxc_b200_add_seek_table_device on `stream` (default: the current stream of the frame's device).  When the
+    tensor has room for the table (zxc_b200_seek_table_device_bound bytes) the call works in place and returns
+    frame[:n]; otherwise it allocates a tensor of that size, copies the frame into it on the stream and returns that.
+    The result is byte for byte what zxc_compress writes with seekable = 1 for the frame's content; a frame that already
+    carries its table comes back unchanged.  Two small reads (the header and footer, then the bound's) size the scratch
+    and the buffer; the stream is synchronised once more to read the result, and a negative one raises ZxcError with
+    its exact code, the frame's bytes unchanged."""
+    if not isinstance(frame, torch.Tensor) or not frame.is_cuda or frame.dtype != torch.uint8 or \
+            not frame.is_contiguous():
+        raise ValueError("frame must be a contiguous uint8 CUDA tensor")
+    f = frame.reshape(-1)
+    cap = f.numel()
+    n = cap if frame_size is None else int(frame_size)
+    if not 0 <= n <= cap:
+        raise ValueError(f"frame_size {n} is outside the tensor's {cap} bytes")
+    dev = f.device
+    with torch.cuda.device(dev):
+        stream = stream or torch.cuda.current_stream(dev)
+        with torch.cuda.stream(stream):
+            # the header's block-size code and the footer's size give the blocks a table would list
+            bs, footer = 4096, 0
+            if n >= 36:
+                h = torch.cat([f[5:6], f[n - 12:n - 4]]).cpu().numpy().tobytes()
+                bs, footer = 1 << h[0] if 12 <= h[0] <= 21 else 4096, int.from_bytes(h[1:], "little")
+            # a chain of more blocks than ceil(footer / bs) is rejected whatever the scratch holds
+            max_blocks = min(-(-footer // bs), max(n - 36, 0) // 8, SEEK_TABLE_MAX_BLOCKS)
+            scratch_size = int(lib.zxc_b200_seek_table_device_scratch_size(n, max_blocks))
+            if scratch_size == 0:
+                raise ValueError("zxc_b200_seek_table_device_scratch_size: frame too large, or no device")
+            bound = int(lib.zxc_b200_seek_table_device_bound(f.data_ptr(), n, stream.cuda_stream)) if n >= 36 else 0
+            out = f
+            if bound > cap:
+                out = torch.empty(bound, dtype=torch.uint8, device=dev)
+                out[:n].copy_(f[:n])
+            scratch = torch.empty(scratch_size, dtype=torch.uint8, device=dev)
+            result = torch.empty(1, dtype=torch.int64, device=dev)
+            rc = lib.zxc_b200_add_seek_table_device(out.data_ptr(), n, out.numel(), scratch.data_ptr(), scratch_size,
+                                                    result.data_ptr(), stream.cuda_stream)
+            if rc != 0:
+                raise ZxcError(rc, "zxc_b200_add_seek_table_device")
+            stream.synchronize()
+            r = int(result.item())
+    if r < 0:
+        raise ZxcError(r, "zxc_b200_add_seek_table_device")
+    return out[:r]
 
 
 class SeekableFrame:
