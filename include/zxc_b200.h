@@ -509,6 +509,33 @@ typedef struct {
  * same bytes, and when there is no device or an allocation fails. */
 ZXC_EXPORT zxc_b200_seekable_device* zxc_b200_seekable_device_open(const void* d_src, uint64_t src_size, void* stream);
 
+/* Opens the seekable frame h_src[0 .. src_size) in page-locked host memory into the same handle type: every call below
+ * takes it as it takes a device handle, and decodes into device memory.  The frame is borrowed like
+ * zxc_seekable_open's src: it must stay valid, page-locked and unchanged while the handle, or any graph captured on it,
+ * is in use; _free does not touch it.  It must be memory the current device can read: from cudaHostAlloc /
+ * cudaMallocHost (torch.Tensor.pin_memory()), or inside a cudaHostRegister range; the call does not register pageable
+ * memory itself.  Synchronous: the SEK table is parsed where it lies, and its block offsets are uploaded once, on
+ * `stream`, to memory the handle owns on the current device, to which the handle is bound.  Returns NULL exactly where
+ * zxc_seekable_open returns NULL for the same bytes, when there is no device, when h_src[0 .. src_size) is not
+ * page-locked memory mapped for the current device (pageable memory gives NULL), and when an allocation fails.
+ * A range call on this handle pulls only the compressed bytes of the blocks its ranges cover over PCIe, into a staging
+ * area in the scratch, and decodes them from there; it differs from the device handle's call only in this:
+ *   - its scratch (zxc_b200_seekable_device_scratch_size) adds the staging area, (J + 2 x max_ranges) x max_comp +
+ *     48 x max_ranges bytes rounded up to 256.  J is the job table's size: ceil(max_bytes / block_size), plus max_ranges
+ *     when the frame's last block is short (a range may cover it whole for fewer than block_size bytes); max_comp is
+ *     the largest on-disk block size the frame's table lists (block_size + 12 at most for frames the reference's
+ *     encoder writes).  So every call of at most max_ranges ranges whose lengths add up to at most max_bytes is
+ *     admitted whole, whatever the frame's block sizes.  Example: a frame of 4 GiB in 64 KiB blocks (last block
+ *     full) with max_comp = 65 548; 1 024 ranges of 4 KiB give J = 64 and stage into (64 + 2 048) x 65 548 + 49 152
+ *     bytes, about 132 MiB, on top of the device handle's scratch (the job table then also grows by the J above);
+ *   - each range stages its own span of blocks, so ranges that share a block fetch it once each;
+ *   - nothing outside h_src[0 .. src_size) is read, and the frame needs no readable bytes behind it: the decode kernels
+ *     read the staging area only;
+ *   - kernel launches per call (zxc_b200_launch_count): 9, the device handle's 8 and one fetch kernel, whatever the
+ *     ranges. */
+ZXC_EXPORT zxc_b200_seekable_device* zxc_b200_seekable_device_open_host(const void* h_src, uint64_t src_size,
+                                                                        void* stream);
+
 /* zxc_seekable_set_dict for the device handle: host pointers, the same verdicts in the same order (NULL_INPUT,
  * DICT_TOO_LARGE, DICT_MISMATCH; a rejected call leaves the handle unchanged), then ZXC_ERROR_MEMORY when the device
  * copy cannot be allocated (the previous dictionary is dropped then, as zxc_seekable_set_dict does).  The dictionary and

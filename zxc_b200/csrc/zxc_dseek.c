@@ -5,6 +5,10 @@
  * Open parses the SEK table on the host with the same parser as zxc_seekable_open (zxw_seek_parse), reading the frame
  * through a few device-to-host copies, and keeps the table's block offsets in device memory: the plan that a range
  * call needs, built once per frame.  A range call is then all device work on the caller's stream (zxc_dseek.cuh).
+ *
+ * zxc_b200_seekable_device_open_host opens a frame in page-locked host memory into the same handle: the table is read
+ * where it lies, and the handle also keeps the frame's device address and its largest on-disk block, with which each
+ * range call stages the blocks it covers into its scratch before decoding them.
  */
 #include <stdlib.h>
 #include <string.h>
@@ -34,6 +38,14 @@ static int dseek_fetch(void* ctx, void* dst, size_t len, uint64_t off) {
     return zxg_d2h_sync(dst, f->d_src + off, len, f->stream);
 }
 
+/* seekable_fetch over host memory */
+static int dseek_fetch_host(void* ctx, void* dst, size_t len, uint64_t off) {
+    const dseek_fetch_ctx* f = (const dseek_fetch_ctx*)ctx;
+    if (off > f->size || len > f->size - off) return ZXC_ERROR_SRC_TOO_SMALL;
+    memcpy(dst, f->d_src + off, len);
+    return ZXC_OK;
+}
+
 /* makes the handle's device current; *prev gets the device to restore */
 static int dseek_enter(const zxc_b200_seekable_device* h, int* prev) {
     *prev = zxg_current_device();
@@ -44,11 +56,11 @@ static void dseek_leave(const zxc_b200_seekable_device* h, int prev) {
     if (h->device != prev) zxg_set_device(prev);
 }
 
-zxc_b200_seekable_device* zxc_b200_seekable_device_open(const void* d_src, uint64_t src_size, void* stream) {
-    if (!d_src || src_size == 0 || zxg_init() != ZXC_OK) return NULL;
-    dseek_fetch_ctx f = {(const uint8_t*)d_src, src_size, stream};
+/* the handle for a frame that d_src reads on the device, its table parsed through fetch over f */
+static zxc_b200_seekable_device* dseek_open(const void* d_src, uint64_t src_size, zxw_fetch_fn fetch,
+                                            dseek_fetch_ctx* f, int host, void* stream) {
     zxw_seek_t tab;
-    if (zxw_seek_parse(dseek_fetch, &f, src_size, &tab) != ZXC_OK) return NULL;
+    if (zxw_seek_parse(fetch, f, src_size, &tab) != ZXC_OK) return NULL;
     zxc_b200_seekable_device* h = (zxc_b200_seekable_device*)calloc(1, sizeof *h);
     const size_t offs_bytes = ((size_t)tab.num_blocks + 1) * sizeof(uint64_t);
     if (h) h->d_offs = (uint64_t*)zxg_dev_alloc(offs_bytes);
@@ -65,8 +77,25 @@ zxc_b200_seekable_device* zxc_b200_seekable_device_open(const void* d_src, uint6
     h->g.block_size = tab.block_size;
     h->g.num_blocks = tab.num_blocks;
     h->g.dict_id = tab.dict_id;
+    h->g.src_size = src_size;
+    for (uint32_t b = 0; host && b < tab.num_blocks; b++)
+        if (tab.comp_sizes[b] > h->g.max_comp) h->g.max_comp = tab.comp_sizes[b]; /* >= 8: a block header */
     zxw_seek_free(&tab);
     return h;
+}
+
+zxc_b200_seekable_device* zxc_b200_seekable_device_open(const void* d_src, uint64_t src_size, void* stream) {
+    if (!d_src || src_size == 0 || zxg_init() != ZXC_OK) return NULL;
+    dseek_fetch_ctx f = {(const uint8_t*)d_src, src_size, stream};
+    return dseek_open(d_src, src_size, dseek_fetch, &f, 0, stream);
+}
+
+zxc_b200_seekable_device* zxc_b200_seekable_device_open_host(const void* h_src, uint64_t src_size, void* stream) {
+    if (!h_src || src_size == 0 || zxg_init() != ZXC_OK) return NULL;
+    const void* mapped = zxg_host_mapped(h_src, (size_t)src_size);
+    if (!mapped) return NULL;
+    dseek_fetch_ctx f = {(const uint8_t*)h_src, src_size, stream};
+    return dseek_open(mapped, src_size, dseek_fetch_host, &f, 1, stream);
 }
 
 /* zxc_seekable_set_dict's verdicts and order (zxc_api.c) */
@@ -110,7 +139,11 @@ size_t zxc_b200_seekable_device_scratch_size(const zxc_b200_seekable_device* h, 
                                              uint64_t max_bytes) {
     if (!h) return 0;
     const uint64_t bs = h->g.block_size;
-    return zxg_dseek_scratch_bytes(h->g.block_size, max_ranges, max_bytes / bs + (max_bytes % bs != 0));
+    uint64_t J = max_bytes / bs + (max_bytes % bs != 0);
+    /* a frame in host memory stages per job, so its table leaves no slack: each range may also cover a short last
+     * block whole for fewer than block_size bytes */
+    if (h->g.max_comp && h->g.total % bs) J += max_ranges;
+    return zxg_dseek_scratch_bytes(h->g.block_size, max_ranges, J, h->g.max_comp);
 }
 
 int zxc_b200_seekable_device_decompress_ranges(zxc_b200_seekable_device* h, const zxc_b200_range_t* d_ranges,

@@ -15,6 +15,17 @@
  *
  * The frame's block table (comp_offsets, num_blocks + 1 entries) was uploaded once when the handle was opened; every
  * launch sequence is the same whatever the ranges hold.
+ *
+ * A frame in page-locked host memory (zxc_b200_seekable_device_open_host) takes the _host instances of the three plan
+ * kernels and one more launch.  Each admitted range stages one span, the on-disk bytes of its blocks b0 .. b1, which
+ * are contiguous in the frame:
+ *
+ *   zxc_dseek_tiles_host  also the span's staged size, scanned as a third quantity: the span at an offset congruent to
+ *                         its host address mod 16, then DS_STAGE_PAD readable bytes, rounded up to 16
+ *   zxc_dseek_scan_host   also the staged bytes' scan and the admitted ranges' staged total
+ *   zxc_dseek_emit_host   job sources as staging offsets
+ *   zxc_dseek_fetch       the admitted spans from mapped host memory into the staging area, as aligned 16-byte loads
+ *                         over PCIe; then the decodes run on the staging area as they run on an HBM frame
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -31,6 +42,7 @@ struct DSeekState {
     unsigned long long first_over; /* first range whose direct jobs do not fit the table (n_ranges: none) */
     unsigned long long d_real;     /* direct jobs of the ranges in front of it */
     unsigned long long s_real;     /* slot jobs of those ranges */
+    unsigned long long p_real;     /* staged bytes of those ranges (a frame in host memory) */
 };
 #define DS_STATE_BYTES 256
 static_assert(sizeof(DSeekState) <= DS_STATE_BYTES, "DSeekState fits its region");
@@ -41,7 +53,10 @@ struct DSeekRec {
     unsigned int ex_s;       /* slot jobs of the tile's earlier ranges */
     int v;                   /* 1: to decode; else the range's result (0 or a check 1-5 code) */
     unsigned int nd, ns;     /* its direct and slot jobs */
-    unsigned int pad[2];
+    union {
+        unsigned int pad[2];
+        unsigned long long ex_p; /* staged bytes of the tile's earlier ranges (a frame in host memory) */
+    };
 };
 
 struct DSeekArgs {
@@ -60,7 +75,15 @@ struct DSeekArgs {
     unsigned long long total, dst_capacity;
     unsigned int n, J, block_size, slot_stride;
     unsigned int need_dict; /* the frame names a dictionary and none is set */
+    /* a frame in host memory (the _host instances and zxc_dseek_fetch) */
+    const u8* hsrc;             /* the frame, at the device address of its page-locked host memory */
+    u8* stage;                  /* the staging area, 16-byte aligned */
+    unsigned long long* ptiles; /* per tile: staged bytes; the scan turns them into exclusive prefixes */
+    unsigned long long src_size;
 };
+
+/* readable bytes behind each staged span: the decode kernels read up to 8 bytes past a block */
+#define DS_STAGE_PAD 8u
 
 /* expected_block_bytes */
 __device__ __forceinline__ u32 ds_expected(const DSeekArgs& A, u64 b) {
@@ -95,14 +118,27 @@ __device__ __forceinline__ int ds_check(const DSeekArgs& A, const zxc_b200_range
     return 1;
 }
 
-__global__ void __launch_bounds__(ASM_THREADS) zxc_dseek_tiles(const DSeekArgs A) {
+/* where a staged span starts: the span [offs[b0], offs[b1 + 1]) of the frame at an offset congruent to its host address
+ * mod 16, so that every copy of zxc_dseek_fetch is an aligned 16-byte copy */
+__device__ __forceinline__ u32 ds_stage_skew(const DSeekArgs& A, u64 off) { return (u32)((uintptr_t)(A.hsrc + off) & 15u); }
+
+/* a range's staged bytes: its span's skew, the span, DS_STAGE_PAD, rounded up to 16 */
+__device__ __forceinline__ u64 ds_stage_bytes(const DSeekArgs& A, const DSeekSpan& s) {
+    const u64 o0 = A.offs[s.b0], o1 = A.offs[s.b1 + 1];
+    return (ds_stage_skew(A, o0) + (o1 - o0) + DS_STAGE_PAD + 15u) & ~(u64)15;
+}
+
+template <bool HOST>
+__device__ __forceinline__ void ds_tiles(const DSeekArgs& A) {
     const u64 base = (u64)blockIdx.x * ASM_TILE + threadIdx.x * ASM_ITEMS;
     u32 nd[ASM_ITEMS], ns[ASM_ITEMS];
     int v[ASM_ITEMS];
-    u64 sd = 0, ss = 0;
+    u64 np[ASM_ITEMS];
+    u64 sd = 0, ss = 0, sp = 0;
 #pragma unroll
     for (u32 k = 0; k < ASM_ITEMS; k++) {
         nd[k] = ns[k] = 0;
+        np[k] = 0;
         v[k] = 0;
         if (base + k < A.n) {
             const zxc_b200_range_t r = A.ranges[base + k];
@@ -111,14 +147,18 @@ __global__ void __launch_bounds__(ASM_THREADS) zxc_dseek_tiles(const DSeekArgs A
                 const DSeekSpan s = ds_span(A, r.offset, r.len);
                 nd[k] = (u32)(s.b1 + 1 - s.tail - s.lo);
                 ns[k] = s.head + s.tail;
+                if constexpr (HOST) np[k] = ds_stage_bytes(A, s);
             }
         }
         sd += nd[k];
         ss += ns[k];
+        sp += np[k];
     }
-    unsigned long long td, ts;
+    unsigned long long td, ts, tp = 0;
     u64 ed = asm_cta_excl(sd, &td);
     u64 es = asm_cta_excl(ss, &ts);
+    u64 ep = 0;
+    if constexpr (HOST) ep = asm_cta_excl(sp, &tp);
 #pragma unroll
     for (u32 k = 0; k < ASM_ITEMS; k++) {
         if (base + k < A.n) {
@@ -128,30 +168,45 @@ __global__ void __launch_bounds__(ASM_THREADS) zxc_dseek_tiles(const DSeekArgs A
             R.v = v[k];
             R.nd = nd[k];
             R.ns = ns[k];
-            R.pad[0] = R.pad[1] = 0;
+            if constexpr (HOST) R.ex_p = ep;
+            else R.pad[0] = R.pad[1] = 0;
             A.recs[base + k] = R;
         }
         ed += nd[k];
         es += ns[k];
+        ep += np[k];
     }
     if (threadIdx.x == 0) {
         A.tiles[2 * blockIdx.x] = td;
         A.tiles[2 * blockIdx.x + 1] = ts;
+        if constexpr (HOST) A.ptiles[blockIdx.x] = tp;
     }
 }
 
-__global__ void __launch_bounds__(ASM_SCAN_THREADS) zxc_dseek_scan(const DSeekArgs A) {
+__global__ void __launch_bounds__(ASM_THREADS) zxc_dseek_tiles(const DSeekArgs A) { ds_tiles<false>(A); }
+/* the staged sizes take 16 more registers than 64 hold; a grid of one CTA per 2 048 ranges needs no occupancy */
+__global__ void __launch_bounds__(ASM_THREADS, 1) zxc_dseek_tiles_host(const DSeekArgs A) { ds_tiles<true>(A); }
+
+template <bool HOST>
+__device__ __forceinline__ void ds_scan(const DSeekArgs& A) {
     __shared__ unsigned long long s_tile, s_first;
     DSeekState* S = A.st;
     const u32 n_tiles = (A.n + ASM_TILE - 1) / ASM_TILE;
     if (threadIdx.x == 0) s_tile = s_first = ~0ull;
-    unsigned long long cd = 0, cs = 0;
+    unsigned long long cd = 0, cs = 0, cp = 0;
     for (u32 b = 0; b < n_tiles; b += blockDim.x) {
         const u32 i = b + threadIdx.x;
         const unsigned long long vd = i < n_tiles ? A.tiles[2 * i] : 0, vs = i < n_tiles ? A.tiles[2 * i + 1] : 0;
         unsigned long long td, ts;
         const unsigned long long ed = cd + asm_cta_excl(vd, &td); /* its barriers also order s_tile */
         const unsigned long long es = cs + asm_cta_excl(vs, &ts);
+        if constexpr (HOST) {
+            const unsigned long long vp = i < n_tiles ? A.ptiles[i] : 0;
+            unsigned long long tp;
+            const unsigned long long ep = cp + asm_cta_excl(vp, &tp);
+            if (i < n_tiles) A.ptiles[i] = ep;
+            cp += tp;
+        }
         if (i < n_tiles) {
             A.tiles[2 * i] = ed;
             A.tiles[2 * i + 1] = es;
@@ -176,17 +231,28 @@ __global__ void __launch_bounds__(ASM_SCAN_THREADS) zxc_dseek_scan(const DSeekAr
         const DSeekRec R = A.recs[f];
         d_real = A.tiles[2 * t] + R.ex_d;
         s_real = A.tiles[2 * t + 1] + R.ex_s;
+        if constexpr (HOST) cp = A.ptiles[t] + R.ex_p;
     }
     S->first_over = f;
     S->d_real = d_real;
     S->s_real = s_real;
+    if constexpr (HOST) S->p_real = cp;
     /* counter 0 claims job indices from the first real job; counters 1 and 2 as in zxc_dplan_place */
     S->ctr[0][0] = A.J - d_real;
     S->ctr[1][0] = 2ull * A.n - s_real;
     S->ctr[0][1] = S->ctr[0][2] = S->ctr[1][1] = S->ctr[1][2] = 0;
 }
 
-__global__ void __launch_bounds__(DS_THREADS) zxc_dseek_emit(const DSeekArgs A) {
+__global__ void __launch_bounds__(ASM_SCAN_THREADS) zxc_dseek_scan(const DSeekArgs A) { ds_scan<false>(A); }
+__global__ void __launch_bounds__(ASM_SCAN_THREADS) zxc_dseek_scan_host(const DSeekArgs A) { ds_scan<true>(A); }
+
+/* a staged range's first span byte in the staging area */
+__device__ __forceinline__ u64 ds_stage_pos(const DSeekArgs& A, u64 i, const DSeekRec& R, const DSeekSpan& s) {
+    return A.ptiles[i / ASM_TILE] + R.ex_p + ds_stage_skew(A, A.offs[s.b0]);
+}
+
+template <bool HOST>
+__device__ __forceinline__ void ds_emit(const DSeekArgs& A) {
     const DSeekState* S = A.st;
     const u64 f = S->first_over, d_real = S->d_real, s_real = S->s_real;
     const u64 d_lead = A.J - d_real, s_lead = 2ull * A.n - s_real;
@@ -205,10 +271,13 @@ __global__ void __launch_bounds__(DS_THREADS) zxc_dseek_emit(const DSeekArgs A) 
     const u64 pd = d_lead + A.tiles[2 * t] + R.ex_d;
     const u64 ps = s_lead + A.tiles[2 * t + 1] + R.ex_s;
     const u64 bs = A.block_size;
+    /* a frame in HBM is read where it lies; a frame in host memory from the range's staged span */
+    u64 rebase = 0;
+    if constexpr (HOST) rebase = ds_stage_pos(A, i, R, s) - A.offs[s.b0];
     for (u32 k = lane; k < R.nd; k += 32) {
         const u64 b = s.lo + k;
         zxc_b200_job_t Jb;
-        Jb.src_off = A.offs[b];
+        Jb.src_off = A.offs[b] + rebase;
         Jb.src_len = (u32)(A.offs[b + 1] - A.offs[b]);
         Jb.dst_off = r.dst_off + (b * bs - r.offset); /* covered whole: the block starts inside the range */
         Jb.dst_cap = ds_expected(A, b);
@@ -217,11 +286,91 @@ __global__ void __launch_bounds__(DS_THREADS) zxc_dseek_emit(const DSeekArgs A) 
     if (lane < R.ns) { /* the head slot comes first, in block order */
         const u64 b = (lane == 0 && s.head) ? s.b0 : s.b1;
         zxc_b200_job_t Jb;
-        Jb.src_off = A.offs[b];
+        Jb.src_off = A.offs[b] + rebase;
         Jb.src_len = (u32)(A.offs[b + 1] - A.offs[b]);
         Jb.dst_off = (ps + lane) * A.slot_stride;
         Jb.dst_cap = ds_expected(A, b);
         A.sjobs[ps + lane] = Jb;
+    }
+}
+
+__global__ void __launch_bounds__(DS_THREADS) zxc_dseek_emit(const DSeekArgs A) { ds_emit<false>(A); }
+__global__ void __launch_bounds__(DS_THREADS) zxc_dseek_emit_host(const DSeekArgs A) { ds_emit<true>(A); }
+
+/* The admitted ranges' staged spans, [0, p_real) of the staging area, copied from the frame in mapped host memory.
+ * CTAs take tiles of DS_FETCH_TILE staged bytes, grid-stride; thread 0 finds the first and the last range a tile
+ * touches by binary search over the scanned staged sizes, and a thread whose chunk lies in a tile of several ranges
+ * searches between those two.  Each thread writes DS_FETCH_UNROLL 16-byte chunks, adjacent threads adjacent chunks,
+ * with all its loads issued before its first store, so that enough reads are in flight to cover PCIe's latency.  A
+ * span sits at an offset congruent to its host address mod 16, so every chunk is one aligned 16-byte load: the
+ * frame's bytes next to the span come along at its two edges, and only where such a chunk would reach past the frame
+ * are its span bytes read one at a time.  Chunks behind a span (its pad) are zeros. */
+#define DS_FETCH_THREADS 256
+#define DS_FETCH_UNROLL 4
+#define DS_FETCH_TILE (DS_FETCH_THREADS * DS_FETCH_UNROLL * 16)
+
+/* the last range in [lo, hi] whose staging starts at or before x, given that lo's does */
+__device__ __forceinline__ u32 ds_stage_find(const DSeekArgs& A, u64 x, u32 lo, u32 hi) {
+    while (lo < hi) {
+        const u32 mid = lo + (hi - lo + 1) / 2;
+        if (A.ptiles[mid / ASM_TILE] + A.recs[mid].ex_p <= x) lo = mid;
+        else hi = mid - 1;
+    }
+    return lo;
+}
+
+__global__ void __launch_bounds__(DS_FETCH_THREADS) zxc_dseek_fetch(const DSeekArgs A) {
+    __shared__ u32 s_lo, s_hi;
+    const DSeekState* S = A.st;
+    const u64 total = S->p_real;
+    const u32 last = (u32)S->first_over - 1; /* every staged byte belongs to a range in front of first_over */
+    for (u64 t0 = (u64)blockIdx.x * DS_FETCH_TILE; t0 < total; t0 += (u64)gridDim.x * DS_FETCH_TILE) {
+        const u64 t1 = t0 + DS_FETCH_TILE < total ? t0 + DS_FETCH_TILE : total;
+        __syncthreads(); /* the previous tile's readers of s_lo, s_hi are done */
+        if (threadIdx.x == 0) {
+            s_lo = ds_stage_find(A, t0, 0, last);
+            s_hi = ds_stage_find(A, t1 - 1, s_lo, last);
+        }
+        __syncthreads();
+        const u32 lo = s_lo, hi = s_hi;
+        u32 ci = ~0u;      /* the range whose span the thread has in hand */
+        u64 c_pos = 0;     /* its first span byte in the staging area */
+        u64 c_len = 0;     /* its span's length */
+        u64 c_src = 0;     /* its span's offset in the frame */
+        uint4 v[DS_FETCH_UNROLL];
+#pragma unroll
+        for (u32 k = 0; k < DS_FETCH_UNROLL; k++) {
+            v[k] = make_uint4(0u, 0u, 0u, 0u);
+            const u64 c = t0 + (u64)(threadIdx.x + k * DS_FETCH_THREADS) * 16;
+            if (c >= t1) continue;
+            const u32 i = lo == hi ? lo : ds_stage_find(A, c, lo, hi);
+            if (i != ci) {
+                ci = i;
+                const DSeekRec R = A.recs[i];
+                const zxc_b200_range_t r = A.ranges[i];
+                const DSeekSpan s = ds_span(A, r.offset, r.len);
+                c_src = A.offs[s.b0];
+                c_len = A.offs[s.b1 + 1] - c_src;
+                c_pos = ds_stage_pos(A, i, R, s);
+            }
+            if (c + 16 <= c_pos || c >= c_pos + c_len) continue; /* the pad */
+            const u64 h = c_src + c - c_pos;                     /* c_src >= 16 > c_pos - c: no wrap */
+            if (h + 16 <= A.src_size) {
+                v[k] = *(const uint4*)(A.hsrc + h);
+            } else { /* the chunk reaches past the frame: the span's bytes alone */
+                u8 b[16];
+#pragma unroll
+                for (u32 j = 0; j < 16; j++) b[j] = (c + j >= c_pos && c + j < c_pos + c_len) ? A.hsrc[h + j] : (u8)0;
+                v[k] = make_uint4(b[0] | b[1] << 8 | b[2] << 16 | (u32)b[3] << 24, b[4] | b[5] << 8 | b[6] << 16 | (u32)b[7] << 24,
+                                  b[8] | b[9] << 8 | b[10] << 16 | (u32)b[11] << 24,
+                                  b[12] | b[13] << 8 | b[14] << 16 | (u32)b[15] << 24);
+            }
+        }
+#pragma unroll
+        for (u32 k = 0; k < DS_FETCH_UNROLL; k++) {
+            const u64 c = t0 + (u64)(threadIdx.x + k * DS_FETCH_THREADS) * 16;
+            if (c < t1) *(uint4*)(A.stage + c) = v[k];
+        }
     }
 }
 

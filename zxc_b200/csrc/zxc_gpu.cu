@@ -2333,6 +2333,21 @@ extern "C" int zxg_h2d_sync(void* d_dst, const void* h_src, size_t bytes, void* 
     return ZXC_OK;
 }
 
+extern "C" const void* zxg_host_mapped(const void* h, size_t bytes) {
+    /* both ends of the frame: page-locked (cudaHostAlloc, or cudaHostRegister of a range that holds it), mapped for the
+     * current device, and one mapping */
+    cudaPointerAttributes a0, a1;
+    const u8* end = (const u8*)h + bytes - 1;
+    if (cudaPointerGetAttributes(&a0, h) != cudaSuccess || cudaPointerGetAttributes(&a1, end) != cudaSuccess) {
+        cudaGetLastError();
+        return NULL;
+    }
+    if (a0.type != cudaMemoryTypeHost || a1.type != cudaMemoryTypeHost || !a0.devicePointer || !a1.devicePointer ||
+        (const u8*)a1.devicePointer - (const u8*)a0.devicePointer != (ptrdiff_t)(bytes - 1))
+        return NULL;
+    return a0.devicePointer;
+}
+
 extern "C" void* zxg_dev_alloc(size_t bytes) {
     void* d = NULL;
     if (cudaMalloc(&d, bytes) != cudaSuccess) {
@@ -2379,20 +2394,27 @@ extern "C" int zxg_ddict_build(void* d_base, const void* h_dict, uint32_t dict_s
  *   slots (2n x round_up(block_size, 16)) | decode scratch (per-warp regions, deferred list)
  * The decode scratch holds the per-warp regions of the larger of the two decode launches, grid_for(max(J, 2n)) warps,
  * so a call with few ranges and few blocks needs no more than its launches use.  total grows with J, and the call
- * takes the largest J whose layout fits the scratch it is given. */
+ * takes the largest J whose layout fits the scratch it is given.
+ * A frame in host memory adds the staged-size tile sums behind the tile sums and the staging area behind the slots:
+ * (J + 2n) x max_comp + DS_STAGE_RANGE n bytes.  A range admitted by the job table stages its nd + ns blocks of at most
+ * max_comp bytes each, plus a skew below 16, DS_STAGE_PAD and rounding to 16 (at most 38 bytes), and the admitted
+ * ranges hold at most J direct and 2n slot jobs: the staging area never decides which ranges are admitted. */
 struct DSeekLayout {
-    size_t recs, tiles, sjobs, sstatus, djobs, dstatus, slots, dec, dec_bytes, total;
+    size_t recs, tiles, ptiles, sjobs, sstatus, djobs, dstatus, slots, stage, dec, dec_bytes, total;
     u32 J, stride;
 };
 #define DS_J_MAX 0x7FFFFFFFu
 #define DS_RANGES_MAX (1u << 30) /* the slot table's 2n entries stay below 2^31 */
+#define DS_STAGE_RANGE 48u
 
-static void ds_layout(u32 bs, u32 n, u32 J, DSeekLayout* L) {
+static void ds_layout(u32 bs, u32 n, u32 J, u32 max_comp, DSeekLayout* L) {
     size_t o = DS_STATE_BYTES;
     L->recs = o;
     o += r256((size_t)n * sizeof(DSeekRec));
     L->tiles = o;
     o += r256(((size_t)n + ASM_TILE - 1) / ASM_TILE * 16);
+    L->ptiles = o;
+    if (max_comp) o += r256(((size_t)n + ASM_TILE - 1) / ASM_TILE * 8);
     L->sjobs = o;
     o += r256((size_t)2 * n * sizeof(zxc_b200_job_t));
     L->sstatus = o;
@@ -2404,33 +2426,40 @@ static void ds_layout(u32 bs, u32 n, u32 J, DSeekLayout* L) {
     L->stride = (bs + 15u) & ~15u;
     L->slots = o;
     o += r256((size_t)2 * n * L->stride);
+    L->stage = o;
+    L->J = J;
+    if (max_comp && ((size_t)J + 2ull * n) > (SIZE_MAX >> 2) / max_comp) { /* a size no scratch has */
+        L->total = SIZE_MAX;
+        return;
+    }
+    if (max_comp) o += r256(((size_t)J + 2ull * n) * max_comp + (size_t)DS_STAGE_RANGE * n);
     L->dec = o;
     L->dec_bytes = launch_scratch_bytes(J > 2 * n ? J : 2 * n, bs);
     L->total = o + L->dec_bytes + 256; /* base alignment slack */
-    L->J = J;
 }
 
-extern "C" size_t zxg_dseek_scratch_bytes(uint32_t block_size, uint32_t n_ranges, uint64_t J) {
+extern "C" size_t zxg_dseek_scratch_bytes(uint32_t block_size, uint32_t n_ranges, uint64_t J, uint32_t max_comp) {
     if (zxg_init() != ZXC_OK || J > DS_J_MAX || n_ranges > DS_RANGES_MAX) return 0;
     DSeekLayout L;
-    ds_layout(block_size, n_ranges, J < 1 ? 1u : (u32)J, &L);
-    return L.total;
+    ds_layout(block_size, n_ranges, J < 1 ? 1u : (u32)J, max_comp, &L);
+    return L.total == SIZE_MAX ? 0 : L.total;
 }
 
 extern "C" int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_ranges, uint32_t n_ranges, void* d_dst,
                                 uint64_t dst_capacity, void* d_scratch, size_t scratch_size, int64_t* d_results,
                                 void* stream) {
-    const u32 bs = h->block_size, n = n_ranges;
+    const u32 bs = h->block_size, n = n_ranges, mc = h->max_comp;
+    const bool host = mc != 0;
     if (n > DS_RANGES_MAX) return ZXC_ERROR_MEMORY;
     DSeekLayout L;
-    ds_layout(bs, n, 1, &L);
+    ds_layout(bs, n, 1, mc, &L);
     if (L.total > scratch_size) return ZXC_ERROR_MEMORY;
     /* the largest direct table whose layout fits: L.total grows with J */
     ds_layout(bs, n, (u32)largest_fit(1, DS_J_MAX, [&](u64 J) {
-                  ds_layout(bs, n, (u32)J, &L);
+                  ds_layout(bs, n, (u32)J, mc, &L);
                   return L.total <= scratch_size;
               }),
-              &L);
+              mc, &L);
     cudaStream_t st = (cudaStream_t)stream;
     u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
     DSeekState* S = (DSeekState*)base;
@@ -2455,26 +2484,40 @@ extern "C" int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_
     A.block_size = bs;
     A.slot_stride = L.stride;
     A.need_dict = h->dict_id != 0 && !has_dict;
+    A.hsrc = host ? (const u8*)h->d_src : NULL;
+    A.stage = host ? base + L.stage : NULL;
+    A.ptiles = host ? (unsigned long long*)(base + L.ptiles) : NULL;
+    A.src_size = h->src_size;
     const u32 n_tiles = (n + ASM_TILE - 1) / ASM_TILE;
     /* a warp per range, and enough threads to zero the status words in front of both tables quickly */
     const u64 by_ranges = ((u64)n * 32 + DS_THREADS - 1) / DS_THREADS;
     u64 by_zero = ((u64)L.J + 2ull * n + DS_THREADS * 16 - 1) / (DS_THREADS * 16);
     if (by_zero > 4096) by_zero = 4096;
     const u32 emit_grid = (u32)(by_ranges > by_zero ? by_ranges : by_zero);
-    zxc_dseek_tiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
-    zxc_dseek_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
-    zxc_dseek_emit<<<emit_grid, DS_THREADS, 0, st>>>(A);
-    __atomic_add_fetch(&g_launches, 3, __ATOMIC_RELAXED);
+    if (host) {
+        /* the same plan with staged sources, then the admitted ranges' spans over PCIe: a grid the SMs hold at once */
+        zxc_dseek_tiles_host<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+        zxc_dseek_scan_host<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+        zxc_dseek_emit_host<<<emit_grid, DS_THREADS, 0, st>>>(A);
+        zxc_dseek_fetch<<<(u32)(g_sm_count > 0 ? g_sm_count : 132) * 8u, DS_FETCH_THREADS, 0, st>>>(A);
+        __atomic_add_fetch(&g_launches, 4, __ATOMIC_RELAXED);
+    } else {
+        zxc_dseek_tiles<<<n_tiles, ASM_THREADS, 0, st>>>(A);
+        zxc_dseek_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(A);
+        zxc_dseek_emit<<<emit_grid, DS_THREADS, 0, st>>>(A);
+        __atomic_add_fetch(&g_launches, 3, __ATOMIC_RELAXED);
+    }
     if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
     /* the blocks covered whole, in place; then the partly covered ones into their slots.  Stream order lets the two
      * runs share the per-warp scratch and the deferred list; each has its own counters. */
     u8* dec = base + L.dec;
     const void* dict = has_dict ? h->d_dict : NULL;
     const void* huf = has_dict ? h->d_dict_huf : NULL;
-    int rc = launch_decode(h->d_src, d_dst, A.djobs, L.J, A.dstatus, dict, h->dict_size, huf, dec, L.dec_bytes, bs, 0,
+    const void* src = host ? (const void*)A.stage : h->d_src;
+    int rc = launch_decode(src, d_dst, A.djobs, L.J, A.dstatus, dict, h->dict_size, huf, dec, L.dec_bytes, bs, 0,
                            S->ctr[0], st, 1);
     if (rc != ZXC_OK) return rc;
-    rc = launch_decode(h->d_src, A.slots, A.sjobs, 2 * n, A.sstatus, dict, h->dict_size, huf, dec, L.dec_bytes, bs, 0,
+    rc = launch_decode(src, A.slots, A.sjobs, 2 * n, A.sstatus, dict, h->dict_size, huf, dec, L.dec_bytes, bs, 0,
                        S->ctr[1], st, 1);
     if (rc != ZXC_OK) return rc;
     zxc_dseek_finish<<<n, DS_THREADS, 0, st>>>(A);

@@ -161,14 +161,21 @@ typedef struct {
     const void* d_dict; /* NULL without a dictionary; its 128-byte table right behind it when d_dict_huf is set */
     uint32_t dict_size;
     const void* d_dict_huf;
+    /* a frame in page-locked host memory (zxc_b200_seekable_device_open_host): d_src is its device address, and a range
+     * call stages the blocks it covers first; max_comp is the table's largest on-disk block, 0 for a frame in HBM */
+    uint32_t max_comp;
+    uint64_t src_size;
 } zxg_dseek_t;
 /* synchronous copies on `stream`, and device memory for a handle (zxg_dev_free waits for the current device first) */
 int zxg_d2h_sync(void* h_dst, const void* d_src, size_t bytes, void* stream);
 int zxg_h2d_sync(void* d_dst, const void* h_src, size_t bytes, void* stream);
 void* zxg_dev_alloc(size_t bytes);
 void zxg_dev_free(void* d);
-/* scratch for n_ranges ranges with a direct job table of J entries (0 when that cannot be planned) */
-size_t zxg_dseek_scratch_bytes(uint32_t block_size, uint32_t n_ranges, uint64_t J);
+/* the device address of page-locked host memory h[0 .. bytes) that the current device can read; NULL otherwise */
+const void* zxg_host_mapped(const void* h, size_t bytes);
+/* scratch for n_ranges ranges with a direct job table of J entries, and a staging area for a frame in host memory
+ * whose largest on-disk block is max_comp bytes (0: a frame in HBM); 0 when that cannot be planned */
+size_t zxg_dseek_scratch_bytes(uint32_t block_size, uint32_t n_ranges, uint64_t J, uint32_t max_comp);
 /* enqueues the plan, the two decodes and the finish; ZXC_ERROR_MEMORY for a scratch below one job-table entry */
 int zxg_dseek_ranges(const zxg_dseek_t* h, const zxc_b200_range_t* d_ranges, uint32_t n_ranges, void* d_dst,
                      uint64_t dst_capacity, void* d_scratch, size_t scratch_size, int64_t* d_results, void* stream);

@@ -803,6 +803,8 @@ def decompress_blocks(blocks, sizes, *, safe=False, checksum=False, dict=None, o
 
 lib.zxc_b200_seekable_device_open.restype = C.c_void_p
 lib.zxc_b200_seekable_device_open.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
+lib.zxc_b200_seekable_device_open_host.restype = C.c_void_p
+lib.zxc_b200_seekable_device_open_host.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
 lib.zxc_b200_seekable_device_set_dict.restype = C.c_int
 lib.zxc_b200_seekable_device_set_dict.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
 lib.zxc_b200_seekable_device_num_blocks.restype = C.c_uint32
@@ -893,22 +895,40 @@ def add_seek_table(frame, *, frame_size=None, stream=None):
 
 
 class SeekableFrame:
-    """Random access into a seekable ZXC frame held in a contiguous uint8 CUDA tensor.
+    """Random access into a seekable ZXC frame held in a contiguous uint8 CUDA tensor, or in a contiguous uint8 CPU
+    tensor in page-locked memory (frame.is_pinned(), e.g. from .pin_memory()).
 
-    Opens the frame with zxc_b200_seekable_device_open (the SEK table is parsed once; its block offsets stay on the
-    device) and decodes byte ranges of the decompressed content with zxc_b200_seekable_device_decompress_ranges.  The
-    frame tensor is kept alive and must not change while the object is open.  dict / dict_huf are host bytes, set
-    with zxc_b200_seekable_device_set_dict.  Raises ValueError when the frame is not seekable (where
-    zxc_seekable_open returns NULL) and ZxcError for a rejected dictionary."""
+    Opens the frame with zxc_b200_seekable_device_open, or zxc_b200_seekable_device_open_host for a pinned CPU
+    tensor (the SEK table is parsed once; its block offsets stay on the device), and decodes byte ranges of the
+    decompressed content with zxc_b200_seekable_device_decompress_ranges.  For a CPU frame each call copies only the
+    compressed blocks its ranges cover over PCIe, and the ranges are decoded on `device` (default: the current CUDA
+    device); a CUDA frame is decoded on its own device.  `gather` and `read` return tensors on that device.  The frame
+    tensor is kept alive and must not change while the object is open.  dict / dict_huf are host bytes, set with
+    zxc_b200_seekable_device_set_dict.  Raises ValueError for a frame tensor of another kind (a pageable CPU tensor
+    among them), when the frame is not seekable (where zxc_seekable_open returns NULL), and ZxcError for a rejected
+    dictionary."""
 
-    def __init__(self, frame, dict=None, dict_huf=None):
+    def __init__(self, frame, dict=None, dict_huf=None, device=None):
         self._h = None  # before any check: __del__ runs on a half-made object too
-        if not frame.is_cuda or frame.dtype != torch.uint8 or not frame.is_contiguous():
-            raise ValueError("frame must be a contiguous uint8 CUDA tensor")
+        if frame.dtype != torch.uint8 or not frame.is_contiguous() or frame.device.type not in ("cuda", "cpu"):
+            raise ValueError("frame must be a contiguous uint8 CUDA tensor, or a pinned CPU one")
+        if frame.is_cuda:
+            if device is not None and torch.device(device) != frame.device:
+                raise ValueError(f"a CUDA frame is decoded on its own device {frame.device}, not {device}")
+            dev = frame.device
+        else:
+            if not frame.is_pinned():
+                raise ValueError("a CPU frame must be in page-locked memory: pass frame.pin_memory()")
+            dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+            if dev.type != "cuda":
+                raise ValueError(f"device must be a CUDA device, not {device}")
+            if dev.index is None:
+                dev = torch.device("cuda", torch.cuda.current_device())
         self.frame = frame.reshape(-1)
-        with torch.cuda.device(self.frame.device):
-            h = lib.zxc_b200_seekable_device_open(self.frame.data_ptr(), self.frame.numel(),
-                                                  torch.cuda.current_stream().cuda_stream)
+        self._device = dev
+        open_ = lib.zxc_b200_seekable_device_open if frame.is_cuda else lib.zxc_b200_seekable_device_open_host
+        with torch.cuda.device(dev):
+            h = open_(self.frame.data_ptr(), self.frame.numel(), torch.cuda.current_stream().cuda_stream)
         if not h:
             raise ValueError("not a seekable ZXC frame (or no device)")
         self._h = h
@@ -931,6 +951,11 @@ class SeekableFrame:
     @property
     def n_blocks(self):
         return int(lib.zxc_b200_seekable_device_num_blocks(self._handle()))
+
+    @property
+    def device(self):
+        """the CUDA device the ranges are decoded on, and where gather and read put their tensors"""
+        return self._device
 
     def _handle(self):
         if self._h is None:
@@ -957,13 +982,13 @@ class SeekableFrame:
         offsets and lengths are int64 CUDA tensors of one length; range i lands at the sum of the lengths before it
         (an exclusive cumsum computed on the device).  Returns (out, results) with no synchronisation when `out` is
         given (its size bounds the scratch); without it, the total length is read back once to allocate out.  `out`
-        must be a contiguous uint8 tensor on the frame's device (ValueError otherwise).  The work runs on `stream`
+        must be a contiguous uint8 tensor on self.device (ValueError otherwise).  The work runs on `stream`
         (default: the current stream), which first waits for the current stream; the returned tensors are written on
         `stream`, so a caller reading them on another stream orders it after `stream` first.
         results[i] (int64, on the device) is the range's byte count or a negative zxc_error_t code, exactly what
         zxc_seekable_decompress_range returns for it; the bytes of a failed range are unspecified."""
         h = self._handle()
-        dev = self.frame.device
+        dev = self._device
         if out is not None:
             _check_out(out, dev)
         offsets = offsets.reshape(-1).to(dev, torch.int64)
@@ -1001,7 +1026,7 @@ class SeekableFrame:
     def read(self, offset, length, stream=None):
         """Decode bytes [offset, offset + length) into a new uint8 tensor; synchronises and raises ZxcError with the
         exact code of zxc_seekable_decompress_range on failure."""
-        dev = self.frame.device
+        dev = self._device
         o = torch.tensor([int(offset)], dtype=torch.int64, device=dev)
         n = torch.tensor([int(length)], dtype=torch.int64, device=dev)
         out = torch.empty(int(length), dtype=torch.uint8, device=dev)
