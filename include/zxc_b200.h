@@ -646,6 +646,62 @@ ZXC_EXPORT size_t zxc_b200_seek_table_device_scratch_size(uint64_t frame_size, u
 ZXC_EXPORT int zxc_b200_add_seek_table_device(void* d_buffer, uint64_t frame_size, uint64_t buffer_capacity,
                                               void* d_scratch, size_t scratch_size, int64_t* d_result, void* stream);
 
+/* ---- page out to host memory: a device buffer compressed into a frame in page-locked host memory ---- */
+/* Device scratch for zxc_b200_compress_device_to_host with these options and window (0: invalid options, or no
+ * device).  The window W is `window` rounded up to whole blocks, at least one block, at most src_size rounded up to a
+ * block.  The scratch holds the padded input copy of one window, the staging slots and per-block words of one window,
+ * 4 bytes per block of the whole input for a seekable frame's SEK entries, the dictionary region (a host dictionary
+ * only) and the per-warp encode slots of one window's full resident encode grid; none of it grows with src_size
+ * except the SEK entries.  From the two size queries on an H100 (132 SMs), seekable, 64 KiB blocks, W = 256 MiB:
+ *   input    level  this call's scratch   zxc_b200_compress_device: scratch + output (zxc_compress_bound)
+ *   1 GiB    3      2 576 MiB             4.08 GiB + 1.02 GiB = 5.10 GiB
+ *   1 GiB    6      5 664 MiB             7.19 GiB + 1.02 GiB = 8.21 GiB
+ *   16 GiB   3      2 577 MiB             34.1 GiB + 16.3 GiB = 50.5 GiB
+ *   16 GiB   6      5 665 MiB             37.3 GiB + 16.3 GiB = 53.6 GiB
+ * Most of this call's scratch is the per-warp encode slots of one window's grid; a smaller window or scratch takes
+ * less (and runs slower). */
+ZXC_EXPORT size_t zxc_b200_compress_device_to_host_scratch_size(uint64_t src_size, uint64_t window,
+                                                                const zxc_compress_opts_t* opts);
+
+/* Compress src_size bytes at d_src (device memory) into a complete ZXC frame at h_dst (page-locked host memory), on
+ * `stream`, asynchronously, `window` input bytes per round, with R = ceil(src_size / W) rounds (W as above).  Each
+ * round copies its input into the scratch, encodes it and writes its compressed blocks into h_dst over the mapping;
+ * only compressed bytes cross PCIe, and the device memory used is the scratch, whatever src_size.
+ *   opts       as for zxc_b200_compress_device (a host dictionary is staged once per call)
+ *   h_dst      page-locked host memory mapped for the current device (cudaHostAlloc / pin_memory(), or inside a
+ *              cudaHostRegister range), h_dst[0 .. dst_capacity) one mapping, any alignment
+ *   window     input bytes per round (see the scratch query)
+ *   d_scratch  device scratch; with less than zxc_b200_compress_device_to_host_scratch_size(...) bytes the encode
+ *              runs as many warps as the scratch holds (same output, slower); below one warp's worth the call fails
+ *   d_result   one device int64: the frame size, or ZXC_ERROR_DST_TOO_SMALL when the frame does not fit
+ *              dst_capacity (h_dst[0 .. dst_capacity) is then unspecified)
+ * *d_result and h_dst[0 .. *d_result) equal what zxc_b200_compress_device gives for the same bytes and options, and so
+ * what zxc_compress returns, whatever the window: a seekable frame opens with zxc_b200_seekable_device_open_host as it
+ * lies.  Only d_src[0 .. src_size) is read, at any alignment; nothing outside h_dst[0 .. dst_capacity), the scratch
+ * and *d_result is written, also when the frame does not fit (blocks that would cross the room are not written).
+ * There is no host synchronisation, no allocation and no copy through a host buffer, except the staging of a host
+ * dictionary; without one the call may be captured in a CUDA graph, and a replay reads d_src's current contents.
+ * Calls on different streams with separate scratch may run concurrently.  Kernel launches per call
+ * (zxc_b200_launch_count): 1 + 5 R (per round: encode, three assembly kernels, host writer; then the finish), plus
+ * one dictionary-seeding kernel with a host dictionary.
+ * Returns ZXC_OK once enqueued, or what the host decides, in zxc_b200_compress_device's order: ZXC_ERROR_NULL_INPUT
+ * (also for a NULL h_dst, d_scratch or d_result, or dst_capacity == 0), ZXC_ERROR_DICT_TOO_LARGE,
+ * ZXC_ERROR_BAD_BLOCK_SIZE, ZXC_B200_ERROR_NO_DEVICE, ZXC_ERROR_DST_TOO_SMALL (dst_capacity below header + trailer),
+ * ZXC_ERROR_CORRUPT_DATA (malformed dict_huf), ZXC_B200_ERROR_UNSUPPORTED when h_dst[0 .. dst_capacity) is not
+ * page-locked memory mapped for the current device as one mapping (pageable memory is refused, not registered), then
+ * ZXC_ERROR_MEMORY when the scratch holds less than one warp. */
+ZXC_EXPORT int zxc_b200_compress_device_to_host(const void* d_src, uint64_t src_size, void* h_dst,
+                                                uint64_t dst_capacity, const zxc_compress_opts_t* opts,
+                                                uint64_t window, void* d_scratch, size_t scratch_size,
+                                                int64_t* d_result, void* stream);
+/* The same with a prepared dictionary (NULL: none), as the other _using_dict calls: nothing is staged, no seeding
+ * kernel runs, and the call may be captured in a CUDA graph. */
+ZXC_EXPORT int zxc_b200_compress_device_to_host_using_dict(const void* d_src, uint64_t src_size, void* h_dst,
+                                                           uint64_t dst_capacity, const zxc_compress_opts_t* opts,
+                                                           const zxc_b200_dict_device* dd, uint64_t window,
+                                                           void* d_scratch, size_t scratch_size, int64_t* d_result,
+                                                           void* stream);
+
 /* ---- push streaming in HBM: the device twins of zxc_cstream_* / zxc_dstream_* (include/zxc_pstream.h) ---- */
 typedef struct zxc_b200_cstream_device_s zxc_b200_cstream_device;
 typedef struct zxc_b200_dstream_device_s zxc_b200_dstream_device;

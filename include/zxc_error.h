@@ -38,8 +38,9 @@ typedef enum {
      * CPU fallback behind this library, so codec entry points report this. */
     ZXC_B200_ERROR_NO_DEVICE = -100,
     ZXC_B200_ERROR_CUDA = -101,
-    /* additive: entry point exported for ABI completeness but outside the
-     * hot-path scope of this build (push streaming). */
+    /* additive: memory the call cannot work on, e.g. a host room that is not
+     * page-locked memory mapped for the device
+     * (zxc_b200_compress_device_to_host). */
     ZXC_B200_ERROR_UNSUPPORTED = -102
 } zxc_error_t;
 

@@ -1091,6 +1091,67 @@ int zxc_b200_compress_device_using_dict(const void* d_src, uint64_t src_size, vo
                            d_result, d_jobs, stream);
 }
 
+size_t zxc_b200_compress_device_to_host_scratch_size(uint64_t src_size, uint64_t window,
+                                                     const zxc_compress_opts_t* opts) {
+    int level;
+    size_t bs;
+    uint32_t nb;
+    if (device_opts(src_size, opts, &level, &bs, &nb) != ZXC_OK) return 0;
+    const size_t dict_size = (opts && opts->dict) ? opts->dict_size : 0;
+    const int seekable = opts && opts->seekable && nb > 0;
+    return zxg_c2h_scratch_bytes(src_size, window, (uint32_t)bs, level, nb, (uint32_t)dict_size, seekable);
+}
+
+/* zxc_b200_compress_device's host verdicts, then UNSUPPORTED for a room that is not mapped page-locked memory */
+static int compress_device_to_host(const void* d_src, uint64_t src_size, void* h_dst, uint64_t dst_capacity,
+                                   const zxc_compress_opts_t* opts, const zxc_b200_dict_device* dd, uint64_t window,
+                                   void* d_scratch, size_t scratch_size, int64_t* d_result, void* stream) {
+    if (!h_dst || dst_capacity == 0 || (src_size > 0 && !d_src) || !d_scratch || !d_result) return ZXC_ERROR_NULL_INPUT;
+    int level;
+    size_t block_size;
+    uint32_t nb;
+    int rc = device_opts(src_size, opts, &level, &block_size, &nb);
+    if (rc != ZXC_OK) return rc;
+    rc = device_ready(dd);
+    if (rc != ZXC_OK) return rc;
+    const int checksum = opts ? opts->checksum_enabled : 0;
+    const int seekable = opts ? opts->seekable : 0;
+    zxg_frame_bytes_t fb;
+    memset(&fb, 0, sizeof fb);
+    fb.fixed = frame_fixed_bytes(nb, seekable);
+    fb.dst_capacity = dst_capacity;
+    fb.seekable = seekable && nb > 0;
+    if (dst_capacity < fb.fixed) return ZXC_ERROR_DST_TOO_SMALL;
+    cdict_t c;
+    rc = cdict_resolve(opts, dd, &c);
+    if (rc != ZXC_OK) return rc;
+    void* mapped = (void*)zxg_host_mapped(h_dst, (size_t)dst_capacity);
+    if (!mapped) return ZXC_B200_ERROR_UNSUPPORTED;
+    zxf_write_file_header(fb.header, sizeof fb.header, block_size, checksum, c.id);
+    zxf_write_block_header(fb.eof, sizeof fb.eof, ZXF_BT_EOF, 0);
+    if (fb.seekable) seek_table_header(fb.sek, nb);
+    zxf_write_footer(fb.footer, sizeof fb.footer, src_size, 0, checksum);
+    return zxg_compress_device_to_host(d_src, src_size, mapped, window, (uint32_t)block_size, level, checksum, nb,
+                                       c.dict, c.dict_size, c.huf_lens, c.dd, &fb, d_scratch, scratch_size, d_result,
+                                       stream);
+}
+
+int zxc_b200_compress_device_to_host(const void* d_src, uint64_t src_size, void* h_dst, uint64_t dst_capacity,
+                                     const zxc_compress_opts_t* opts, uint64_t window, void* d_scratch,
+                                     size_t scratch_size, int64_t* d_result, void* stream) {
+    return compress_device_to_host(d_src, src_size, h_dst, dst_capacity, opts, NULL, window, d_scratch, scratch_size,
+                                   d_result, stream);
+}
+
+int zxc_b200_compress_device_to_host_using_dict(const void* d_src, uint64_t src_size, void* h_dst,
+                                                uint64_t dst_capacity, const zxc_compress_opts_t* opts,
+                                                const zxc_b200_dict_device* dd, uint64_t window, void* d_scratch,
+                                                size_t scratch_size, int64_t* d_result, void* stream) {
+    zxc_compress_opts_t t;
+    return compress_device_to_host(d_src, src_size, h_dst, dst_capacity, copts_no_dict(opts, &t), dd, window,
+                                   d_scratch, scratch_size, d_result, stream);
+}
+
 size_t zxc_b200_compress_device_batch_scratch_size(uint32_t max_frames, uint64_t max_total_src,
                                                    const zxc_compress_opts_t* opts) {
     int level;

@@ -25,6 +25,7 @@
 #include "zxc_decode.cuh"
 #include "zxc_encode.cuh"
 #include "zxc_assemble.cuh"
+#include "zxc_c2host.cuh"
 #include "zxc_dbatch.cuh"
 #include "zxc_cbatch.cuh"
 #include "zxc_dplan.cuh"
@@ -1156,21 +1157,13 @@ static int enc_stage_dict(EncodeParams& P, u8* d_dict, const void* h_dict, u32 d
     return rc;
 }
 
-static int launch_encode(const EncLaunch& E, cudaStream_t st) {
-    EncodeParams P;
+/* The encode kernel on E's blocks with the dictionary fields already in P (staged once for several launches) */
+static int launch_encode_staged(EncodeParams P, const EncLaunch& E, cudaStream_t st) {
     P.src = E.d_src;
     P.staging = E.d_stage;
     P.out_size = E.d_sizes;
     P.scratch = E.d_scratch;
     P.counter = E.counter;
-    P.dict = NULL;
-    P.seed_head = NULL;
-    P.seed_chain = NULL;
-    P.dict_huf_lens = NULL;
-    if (E.dd || (E.h_dict && E.dict_size)) {
-        const int rc = enc_stage_dict(P, E.d_dict, E.h_dict, E.dict_size, E.level, E.h_dict_huf_lens, E.dd, true, st);
-        if (rc != ZXC_OK) return rc;
-    }
     P.src_size = E.src_size;
     P.scratch_stride = enc_layout(E.block_size, E.level).total;
     P.block_size = E.block_size;
@@ -1186,6 +1179,24 @@ static int launch_encode(const EncLaunch& E, cudaStream_t st) {
     else zxc_encode_kernel<false><<<grid, threads, 0, st>>>(P);
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+static EncodeParams enc_no_dict(void) {
+    EncodeParams P;
+    P.dict = NULL;
+    P.seed_head = NULL;
+    P.seed_chain = NULL;
+    P.dict_huf_lens = NULL;
+    return P;
+}
+
+static int launch_encode(const EncLaunch& E, cudaStream_t st) {
+    EncodeParams P = enc_no_dict();
+    if (E.dd || (E.h_dict && E.dict_size)) {
+        const int rc = enc_stage_dict(P, E.d_dict, E.h_dict, E.dict_size, E.level, E.h_dict_huf_lens, E.dd, true, st);
+        if (rc != ZXC_OK) return rc;
+    }
+    return launch_encode_staged(P, E, st);
 }
 
 /* gather the staging slots to out + dst_off[j] */
@@ -1358,6 +1369,119 @@ extern "C" int zxg_compress_device(const void* d_src, uint64_t src_size, void* d
         launch_compact(d_stage, F.staging_stride, d_offs, d_sizes, d_dst8 + 16 /* file header */, n_blocks, st);
     }
     zxc_asm_finish<<<1, 1, 0, st>>>(d_dst8, state, F, (long long*)d_result);
+    __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
+    return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
+}
+
+/* ------------------------------------------------------------------------- */
+/* device buffer to a frame in page-locked host memory, window by window     */
+/* (zxc_b200_compress_device_to_host: kernels in zxc_c2host.cuh)             */
+/* ------------------------------------------------------------------------- */
+/* Scratch layout, from the caller's base rounded up to 256 bytes (every region 256-aligned), for windows of wb blocks:
+ *   C2hState (256) | input copy of one window + 64 zero bytes | dictionary region (with a host dictionary) |
+ *   staging slots (wb) | sizes (u32 x wb) | body offsets (u64 x wb) | tile sums (u64 per ASM_TILE of wb) |
+ *   SEK entries (u32 x n, seekable only) | per-warp encode slots */
+static DevEncLayout c2h_layout(u64 W, u32 block_size, u32 n_blocks, int level, u32 dict_size, int seekable,
+                               size_t* sek) {
+    const u32 wb = (u32)(W / block_size);
+    DevEncLayout L = dev_enc_layout(W, block_size, wb, level, dict_size);
+    *sek = L.warps;
+    if (seekable) L.warps += r256((size_t)n_blocks * 4);
+    L.fixed = L.warps + 256;
+    return L;
+}
+
+/* window rounded up to whole blocks, capped at the input rounded up to a block, at least one block */
+static u64 c2h_window(uint64_t src_size, uint64_t window, u32 block_size) {
+    const u64 cap = (src_size + block_size - 1) / block_size * block_size;
+    u64 W = window / block_size + (window % block_size != 0);
+    W = W > (cap / block_size) ? cap : W * block_size;
+    return W < block_size ? block_size : W;
+}
+
+extern "C" size_t zxg_c2h_scratch_bytes(uint64_t src_size, uint64_t window, uint32_t block_size, int level,
+                                        uint32_t n_blocks, uint32_t dict_size, int seekable) {
+    if (zxg_init() != ZXC_OK) return 0;
+    const u64 W = c2h_window(src_size, window, block_size);
+    size_t sek;
+    const DevEncLayout L = c2h_layout(W, block_size, n_blocks, level, dict_size, seekable, &sek);
+    return L.fixed + (size_t)enc_full_warps((u32)(W / block_size)) * L.wstride;
+}
+
+extern "C" int zxg_compress_device_to_host(const void* d_src, uint64_t src_size, void* h_mapped, uint64_t window,
+                                           uint32_t block_size, int level, int checksum, uint32_t n_blocks,
+                                           const void* h_dict, uint32_t dict_size, const uint8_t* h_dict_huf_lens,
+                                           const zxg_ddict_t* dd, const zxg_frame_bytes_t* fb, void* d_scratch,
+                                           size_t scratch_size, int64_t* d_result, void* stream) {
+    const int irc = zxg_init();
+    if (irc != ZXC_OK) return irc;
+    const u64 W = c2h_window(src_size, window, block_size);
+    const u32 wb = (u32)(W / block_size);
+    size_t sek_off;
+    const DevEncLayout L = c2h_layout(W, block_size, n_blocks, level, dict_size, fb->seekable, &sek_off);
+    if (scratch_size < L.fixed + L.wstride) return ZXC_ERROR_MEMORY;
+    const size_t fit = (scratch_size - L.fixed) / L.wstride;
+    const u32 full = enc_full_warps(wb);
+    const u32 warps = fit < full ? (u32)fit : full;
+    cudaStream_t st = (cudaStream_t)stream;
+    u8* base = (u8*)(((uintptr_t)d_scratch + 255) & ~(uintptr_t)255);
+    C2hState* state = (C2hState*)base;
+    u8* hd = (u8*)h_mapped;
+    u32* d_sek = fb->seekable ? (u32*)(base + sek_off) : NULL;
+    const u32 sstride = enc_staging_stride(block_size);
+    const u32 gmax = (u32)(g_sm_count > 0 ? g_sm_count : 132) * 8u;
+    if (cudaMemsetAsync(state, 0, sizeof(C2hState), st) != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    EncodeParams P = enc_no_dict();
+    if (n_blocks && (dd || (h_dict && dict_size))) { /* staged once for every round */
+        const int rc = enc_stage_dict(P, base + L.dict, h_dict, dict_size, level, h_dict_huf_lens, dd, true, st);
+        if (rc != ZXC_OK) return rc;
+    }
+    C2hHeader H;
+    memcpy(H.b, fb->header, 16);
+    u32 rounds = 0;
+    for (u64 s0 = 0; s0 < src_size; s0 += W, rounds++) {
+        const u64 len = src_size - s0 < W ? src_size - s0 : W;
+        const u32 wn = (u32)((len + block_size - 1) / block_size);
+        const u32 j0 = (u32)(s0 / block_size);
+        u8* d_in = base + L.in;
+        u8* d_stage = base + L.stage;
+        u32* d_sizes = (u32*)(base + L.sizes);
+        unsigned long long* d_offs = (unsigned long long*)(base + L.offs);
+        unsigned long long* d_tiles = (unsigned long long*)(base + L.tiles);
+        const u32 n_tiles = (wn + ASM_TILE - 1) / ASM_TILE;
+        if (cudaMemcpyAsync(d_in, (const u8*)d_src + s0, (size_t)len, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+            cudaMemsetAsync(d_in + len, 0, 64, st) != cudaSuccess)
+            return ZXC_B200_ERROR_CUDA;
+        const EncLaunch E = {d_in, len, block_size, wn, level, checksum, d_stage, d_sizes, base + L.warps,
+                             warps, &state->counter, base + L.dict, h_dict, dict_size, h_dict_huf_lens, dd};
+        const int rc = launch_encode_staged(P, E, st);
+        if (rc != ZXC_OK) return rc;
+        const u64 chunks = ((u64)wn * sstride + 15) / 16 + 1;
+        const u32 wgrid = (u32)((chunks + C2H_THREADS - 1) / C2H_THREADS < gmax ? (chunks + C2H_THREADS - 1) / C2H_THREADS
+                                                                                 : gmax);
+        zxc_asm_tile_sums<<<n_tiles, ASM_THREADS, 0, st>>>(d_sizes, wn, d_tiles);
+        zxc_c2h_scan<<<1, ASM_SCAN_THREADS, 0, st>>>(d_tiles, n_tiles, state, fb->fixed, fb->dst_capacity);
+        zxc_c2h_blocks<<<n_tiles, ASM_THREADS, 0, st>>>(d_sizes, d_stage, d_tiles, d_offs, state, d_sek, wn, j0,
+                                                        n_blocks, sstride, checksum ? 1u : 0u);
+        zxc_c2h_write<<<wgrid, C2H_THREADS, 0, st>>>(hd, d_stage, sstride, d_offs, d_sizes, wn, state, H, rounds & 1u);
+        __atomic_add_fetch(&g_launches, 4, __ATOMIC_RELAXED);
+        if (cudaGetLastError() != cudaSuccess) return ZXC_B200_ERROR_CUDA;
+    }
+    C2hFinish F;
+    memcpy(F.header, fb->header, 16);
+    memcpy(F.eof, fb->eof, 8);
+    memcpy(F.sek, fb->sek, 8);
+    memcpy(F.footer, fb->footer, 12);
+    F.dst_capacity = fb->dst_capacity;
+    F.fixed = fb->fixed;
+    F.n_blocks = n_blocks;
+    F.checksum = checksum ? 1u : 0u;
+    F.seekable = fb->seekable ? 1u : 0u;
+    F.parity = rounds & 1u;
+    const u64 tchunks = (fb->fixed + 31) / 16 + 2; /* the trailer, the carried tail and chunk 0 */
+    const u32 fgrid = (u32)((tchunks + C2H_THREADS - 1) / C2H_THREADS < gmax ? (tchunks + C2H_THREADS - 1) / C2H_THREADS
+                                                                              : gmax);
+    zxc_c2h_finish<<<fgrid, C2H_THREADS, 0, st>>>(hd, (const u8*)d_sek, state, F, (long long*)d_result);
     __atomic_add_fetch(&g_launches, 1, __ATOMIC_RELAXED);
     return cudaGetLastError() == cudaSuccess ? ZXC_OK : ZXC_B200_ERROR_CUDA;
 }

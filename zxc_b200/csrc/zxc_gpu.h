@@ -91,6 +91,18 @@ int zxg_compress_device(const void* d_src, uint64_t src_size, void* d_dst, uint3
                         const uint8_t* h_dict_huf_lens, const zxg_ddict_t* dd, const zxg_frame_bytes_t* fb,
                         void* d_scratch, size_t scratch_size, int64_t* d_result, zxc_b200_job_t* d_jobs, void* stream);
 
+/* Device buffer to a frame in page-locked host memory (zxc_b200_compress_device_to_host; kernels in zxc_c2host.cuh):
+ * the compress above, `window` input bytes per round, with h_mapped the device address of the caller's room.  Scratch
+ * for the full resident encode grid of one window (0 without a device); ZXC_ERROR_MEMORY when the scratch holds less
+ * than one warp. */
+size_t zxg_c2h_scratch_bytes(uint64_t src_size, uint64_t window, uint32_t block_size, int level, uint32_t n_blocks,
+                             uint32_t dict_size, int seekable);
+int zxg_compress_device_to_host(const void* d_src, uint64_t src_size, void* h_mapped, uint64_t window,
+                                uint32_t block_size, int level, int checksum, uint32_t n_blocks, const void* h_dict,
+                                uint32_t dict_size, const uint8_t* h_dict_huf_lens, const zxg_ddict_t* dd,
+                                const zxg_frame_bytes_t* fb, void* d_scratch, size_t scratch_size, int64_t* d_result,
+                                void* stream);
+
 /* The decode options of a device-resident decode, resolved on the host from zxc_decompress_opts_t: what needs no
  * frame bytes. */
 typedef struct {

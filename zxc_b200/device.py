@@ -11,6 +11,8 @@ one zxc_b200_compress_device_batch call.  ``decompress_inplace`` decodes a frame
 into the same buffer with zxc_b200_decompress_inplace_device, and ``load_frame`` uses it to bring a frame from the
 host into HBM and expand it there with no second buffer.  ``compress_blocks`` and ``decompress_blocks`` are the block
 API in HBM: many frameless blocks per zxc_b200_compress_blocks_device / zxc_b200_decompress_blocks_device call.
+``compress_to_host`` compresses a CUDA tensor into a frame in pinned host memory with
+zxc_b200_compress_device_to_host, one window of input per round, so the HBM it takes is bounded by the window.
 ``DeviceDict`` prepares a dictionary in HBM once; passed as ``dict`` to those helpers it makes them call the _using_dict
 entry points, which stage nothing per call.  ``train_dict``, ``train_dict_huf`` and ``dict_train`` train a dictionary on
 samples that are already in HBM (zxc_b200_train_dict_device and its siblings), and ``DeviceDict.train`` makes a
@@ -318,6 +320,72 @@ def compress(src, *, level=0, block_size=0, checksum=False, seekable=False, dict
         return DeviceFrame(dst[:size], jobs, bs, n, bool(checksum), dd.dict, dd.dict_huf)
     return DeviceFrame(dst[:size], jobs, bs, n, bool(checksum), keep[0] if dict is not None else None,
                        keep[1] if dict_huf is not None and dict is not None else None)
+
+
+lib.zxc_b200_compress_device_to_host_scratch_size.restype = C.c_size_t
+lib.zxc_b200_compress_device_to_host_scratch_size.argtypes = [C.c_uint64, C.c_uint64, C.c_void_p]
+lib.zxc_b200_compress_device_to_host.restype = C.c_int
+lib.zxc_b200_compress_device_to_host.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                 C.c_uint64, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
+lib.zxc_b200_compress_device_to_host_using_dict.restype = C.c_int
+lib.zxc_b200_compress_device_to_host_using_dict.argtypes = (lib.zxc_b200_compress_device_to_host.argtypes[:5] +
+                                                            [C.c_void_p] +
+                                                            lib.zxc_b200_compress_device_to_host.argtypes[5:])
+WINDOW_DEFAULT = 256 << 20
+
+
+def compress_to_host(src, *, level=0, block_size=0, checksum=False, seekable=False, dict=None, dict_huf=None,
+                     window=None, out=None, stream=None):
+    """Compress a contiguous CUDA tensor (its bytes) into a ZXC frame in page-locked host memory; returns a uint8 CPU
+    tensor, out[:size].
+
+    Runs zxc_b200_compress_device_to_host on `stream` (default: torch's current stream of src's device): `window`
+    input bytes per round (default 256 MiB) are encoded in HBM and their compressed blocks written straight into
+    `out`, so the device memory taken is bounded by the window, not by src.  `out` is a pinned, contiguous uint8 CPU
+    tensor (default: a fresh pinned tensor of zxc_compress_bound bytes).  The stream is synchronised once to read the
+    frame size.  The frame equals what zxc_compress returns for the same bytes and options.  dict / dict_huf are host
+    bytes, or dict is a DeviceDict (the _using_dict call: nothing is staged).  Raises ValueError for a CPU src or an
+    `out` that is not a pinned contiguous uint8 CPU tensor, and ZxcError with the library's code otherwise.
+
+    The frame round-trips:
+
+        frame = compress_to_host(x, level=3, seekable=True)
+        SeekableFrame(frame).read(0, x.numel())      # ranges decoded from host memory (seekable frames)
+        load_frame(frame)                             # any frame, decoded in HBM
+    """
+    b = _bytes_view(src)
+    n = b.numel()
+    cap = int(lib.zxc_compress_bound(n))
+    if out is not None:
+        if out.device.type != "cpu" or out.dtype != torch.uint8 or not out.is_contiguous() or not out.is_pinned():
+            raise ValueError("out must be a pinned, contiguous uint8 CPU tensor (torch.empty(..., pin_memory=True))")
+        out = out.reshape(-1)
+    o = _Opts(level=level, block_size=block_size, checksum_enabled=int(bool(checksum)), seekable=int(bool(seekable)))
+    keep, dd = _dict_opts(o, dict, dict_huf)
+    window = WINDOW_DEFAULT if window is None else int(window)
+    with torch.cuda.device(b.device):
+        stream = stream or torch.cuda.current_stream(b.device)
+        with torch.cuda.stream(stream):
+            scratch_size = int(lib.zxc_b200_compress_device_to_host_scratch_size(n, window, C.byref(o)))
+            if scratch_size == 0:
+                raise ValueError("zxc_b200_compress_device_to_host_scratch_size: invalid options (level, block_size, "
+                                 "dict) or no device")
+            if out is None:
+                out = torch.empty(cap, dtype=torch.uint8, pin_memory=True)
+            scratch = torch.empty(scratch_size, dtype=torch.uint8, device=b.device)
+            result = torch.empty(1, dtype=torch.int64, device=b.device)
+            rc = _call("zxc_b200_compress_device_to_host", dd,
+                       (b.data_ptr() if n else None, n, out.data_ptr() if out.numel() else None, out.numel(),
+                        C.byref(o)),
+                       (window, scratch.data_ptr(), scratch_size, result.data_ptr(), stream.cuda_stream))
+            if rc != 0:
+                raise ZxcError(rc, "zxc_b200_compress_device_to_host")
+            stream.synchronize()
+            size = int(result.item())
+    del keep
+    if size < 0:
+        raise ZxcError(size, "zxc_b200_compress_device_to_host")
+    return out[:size]
 
 
 def decompress(f, *, verify=False, stream=None):
